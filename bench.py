@@ -1,22 +1,30 @@
 #!/usr/bin/env python3
-"""bench.py -- marker-scan throughput on B200 (BASELINE.json metric: YAML MB/s scanned + markers/s,
+"""bench.py -- marker-scan throughput on H100 (BASELINE.json metric: YAML MB/s scanned + markers/s,
 % of the HBM-read roofline, next to the reference's CPU path).
 
     python bench.py --gpus N --steps K --warmup W            (N>1: launched under torch.distributed.run)
     python bench.py --impl reference ...                     (the reference's CPU path on the host cores)
+    python bench.py ... --dump-outputs DIR                   (also write what the last timed step computed)
 
 A "step" is one pass of the hot path over the whole synthetic batch:
   workload  BASELINE.json configs[3] / the north-star target: 2,621,440 synthetic manifests x 4,096 B
             = 10 GiB (generator: obm_corpus.h, splitmix64(0x0B200 ^ doc index), 8 markers per file),
             resident in HBM, sharded by file over the N ranks ("strong" scaling: total work fixed).
-            Inputs are 10 GiB >> 126 MB L2, so no L2 flush is needed between timed iterations.
+            Inputs are 10 GiB >> 50 MB L2, so no L2 flush is needed between timed iterations.
   value     total input MB / device time of (scan + emit [+ the N>1 index all-gather]), max over ranks
   e2e       the same metric through the C-ABI host entry point obm_lex_batch: pinned host buffers,
             H2D of the manifests and D2H of tuples + offsets inside the timed region (bounded sample)
   roofline  algorithmic bytes = 1 byte read per input byte (SURVEY.md 8d) / time of all scan kernels,
-            against the measured HBM copy peak in MEASURED_PEAKS.json
-  cpu_baseline  the oracle (C restatement of the reference's Go lexer; no Go toolchain here) on all
-            host cores over a bounded sample of the same corpus
+            against the HBM copy peak in MEASURED_PEAKS.json if present, else the H100 SXM data sheet's 3.35 TB/s
+  cpu_baseline  the oracle (C restatement of the reference's Go lexer) on all host cores over a bounded
+            sample of the same corpus
+  gpu       the card's name, power limit and maximum SM clock: every number above belongs to them
+
+--dump-outputs DIR writes, after the timed steps, what the last step left for its caller as float64 .npy files: the
+tuple stream of rank 0's shard (a fixed, seeded sample of its words, split into kind / off / len), the per-document tuple
+offsets (sampled the same way above 2^20 documents), the marker and lexeme counts and the status words; with N > 1 also
+a sample of the all-gathered marker index.  The corpus is a function of the arguments, so two builds run with the same
+arguments can be compared file for file.
 """
 import argparse
 import json
@@ -32,7 +40,8 @@ if ROOT not in sys.path:
 
 DOC_BYTES = 4096
 FULL_DOCS = 2_621_440  # 10 GiB
-FALLBACK_HBM_GBS = 6650.0  # B200_PROFILING.md fallback when MEASURED_PEAKS.json is absent
+FALLBACK_HBM_GBS = 3350.0  # H100 SXM data sheet, used when MEASURED_PEAKS.json is absent
+DUMP_ROWS = 1 << 20  # rows per sampled array of --dump-outputs: 8 B each as float64, under 64 MB in all
 
 
 def measured_peak():
@@ -40,7 +49,47 @@ def measured_peak():
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
     except Exception:
-        return FALLBACK_HBM_GBS, "fallback (B200_PROFILING.md)"
+        return FALLBACK_HBM_GBS, "H100 SXM data sheet (3.35 TB/s), not measured"
+
+
+def gpu_info(gpu_index):
+    """name, power limit and maximum SM clock of the card the numbers are measured on"""
+    try:
+        row = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader,nounits",
+                              "-i", str(gpu_index)], capture_output=True, text=True, timeout=30).stdout.strip().split(",")
+        return {"name": row[0].strip(), "power_limit_w": float(row[1]), "sm_max_mhz": float(row[2])}
+    except Exception:
+        return None
+
+
+def sample_rows(n, k, seed):
+    """sorted row indices: all n rows, or a fixed seeded sample of about k of them"""
+    import numpy as np
+    if n <= k:
+        return np.arange(n, dtype=np.int64)
+    return np.unique(np.random.default_rng(seed).integers(0, n, k, dtype=np.int64))
+
+
+def dump_outputs(out_dir, d_out, n_tuples, d_toff, d_counts, d_status, index=None):
+    """writes what the step left in the caller's buffers as DIR/<name>.npy (float64; a tuple word is split into its
+    kind / off / len fields, include/obmarkers.h, because float64 holds only 53 bits)"""
+    import numpy as np
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    dev = d_out.device
+    ti = sample_rows(n_tuples, DUMP_ROWS, 1)
+    t = d_out[torch.from_numpy(ti).to(dev)].cpu().numpy().view(np.uint64)
+    di = sample_rows(d_toff.numel(), DUMP_ROWS, 2)
+    arrays = {"tuple_index": ti, "tuple_kind": t >> np.uint64(59), "tuple_len": (t >> np.uint64(32)) & np.uint64(0x7FFFFFF),
+              "tuple_off": t & np.uint64(0xFFFFFFFF), "doc_index": di,
+              "doc_tuple_off": d_toff[torch.from_numpy(di).to(dev)].cpu().numpy(),
+              "counts": np.array([n_tuples] + d_counts.cpu().tolist()), "status": d_status.cpu().numpy()}
+    if index is not None:  # N > 1: the all-gathered marker index, records {doc, tuple, off, registry id | scope count << 16}
+        ii = sample_rows(index.shape[0], DUMP_ROWS // 4, 3)
+        arrays["marker_index_row"] = ii
+        arrays["marker_index"] = index[torch.from_numpy(ii).to(dev)].cpu().numpy().view(np.uint32)
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), np.ascontiguousarray(a, dtype=np.float64))
 
 
 class ClockSampler:
@@ -137,7 +186,10 @@ def main():
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--no-cpu", action="store_true")
     ap.add_argument("--mode", type=int, default=0, help="0 auto (fast path), 1 exact path only")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write what the last timed step computed as DIR/<name>.npy (float64)")
     args = ap.parse_args()
+    if args.dump_outputs and args.impl != "b200":
+        ap.error("--dump-outputs writes the outputs of the GPU path (--impl b200)")
     args.warmup = max(args.warmup, 3) if args.impl == "b200" else args.warmup
 
     rank = int(os.environ.get("RANK", "0"))
@@ -150,16 +202,16 @@ def main():
                           f"8 markers/file, sharded by file over {world} rank(s), HBM-resident",
               "docs": args.docs, "doc_bytes": DOC_BYTES, "flavour": args.flavour,
               "parallelism": f"file-shard x{world}; step = scan + emit" + (" + marker index (16 B per registered marker) + one NCCL all-gather of the index records (obm_lex_batch_sharded_device, C ABI)" if world > 1 else ""),
-              "l2": "inputs (>= 1.25 GiB per rank) exceed the 126 MB L2; no flush needed"}
+              "l2": "inputs (>= 1.25 GiB per rank) exceed the 50 MB L2; no flush needed"}
 
     if args.impl == "reference":
         # The reference's own CPU implementation of the path; Go cannot be built here, so this is the
         # oracle port of internal/markers/lexer on all host cores (kind "port").  Rank 0 only.
         if rank != 0:
             return 0
-        # a step = one pass of the CPU path over a BOUNDED SAMPLE of the workload (1 GiB by default: ~1 s per pass on this
-        # box's cores); `config.workload` names the full workload, `config.sample` what a step really covers
-        steps = max(3, min(args.steps, 5))
+        # a step = one pass of the CPU path over a BOUNDED SAMPLE of the workload (1 GiB by default);
+        # `config.workload` names the full workload, `config.sample` what a step really covers
+        steps = args.steps
         ref_docs = max(args.cpu_docs, int(os.environ.get("OBM_BENCH_REF_DOCS", 262144)))
         r = cpu_reference_run(ref_docs, cores, steps, 1, args.flavour)
         config["sample"] = r["sample"]
@@ -276,6 +328,12 @@ def main():
         sampler.start()
     ms = timed(step, args.steps)
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs and rank == 0:
+        index = None
+        if comm is not None:
+            recs = d_idx_all.view(torch.int32).view(-1, 4)
+            index = torch.cat([recs[r * exch["stride"]:r * exch["stride"] + exch["per_rank"][r]] for r in range(world)])
+        dump_outputs(args.dump_outputs, d_out, int(d_toff[-1].item()), d_toff, d_counts, d_status, index)
     launches = (ob._native.lib().obm_launches_last_call(sc.handle) + (2 if world > 1 else 0)) * args.steps  # scan kernels (+ N > 1: the one-pass index = k_flat_tile_docs + k_marker_index_flat)
 
     # the parts, same stream, same events: scan-only time is the roofline's denominator
@@ -354,13 +412,6 @@ def main():
 
     peak, peak_src = measured_peak()
     achieved = (total_bytes / world) / (ms_scan / 1e3) / 1e9  # per-GPU GB/s of algorithmic input bytes
-    traffic = None
-    try:
-        with open(os.path.join(ROOT, "profiles", "traffic.json")) as f:
-            tj = json.load(f)
-            traffic = int(tj["dram_bytes_per_input_byte"] * (total_bytes // world))  # ncu capture scaled to this launch
-    except Exception:
-        pass
     cpu = None
     if not args.no_cpu and world >= 1:
         r = cpu_reference_run(args.cpu_docs, cores, 2, 1, args.flavour)
@@ -374,10 +425,10 @@ def main():
             "tuples": tot_tuples, "tuple_bytes_per_input_byte": tot_tuples * 8 / total_bytes,
             "docs_exact_path": docs_exact, "docs_fatal": docs_fatal, "mode": args.mode,
             "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                         "traffic": traffic, "peak_source": peak_src, "ms_scan_kernels": ms_scan,
+                         "peak_source": peak_src, "ms_scan_kernels": ms_scan,
                          "algorithmic_bytes_per_launch": total_bytes // world,
                          "note": "1 B read per input byte (SURVEY 8d); time = all kernels of one scan, per GPU"},
-            "cpu_baseline": cpu, "e2e": e2e, "gpu_launches": launches, "clocks": clocks,
+            "cpu_baseline": cpu, "e2e": e2e, "gpu_launches": launches, "clocks": clocks, "gpu": gpu_info(local_rank),
             "parts": {"ms_scan": ms_scan, "ms_parse": ms_parse, "results": tot_results, "args": tot_args,
                       "result_bytes_per_input_byte": tot_results * 32 / total_bytes},
             "exchange": ({"in_step": "ncclAllGather of 16-byte marker-index records (+ an 8-byte count gather), through the C ABI",

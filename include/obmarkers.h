@@ -1,5 +1,5 @@
 /*
- * obmarkers.h -- C ABI of libobmarkers.so, the B200 (sm_100a) marker scanner.
+ * obmarkers.h -- C ABI of libobmarkers.so, the H100 (sm_90a) marker scanner.
  *
  * Drop-in boundary for the marker-scanning hot path of vmware-tanzu-labs/operator-builder
  * (reference @ 2827f233; file:line citations are relative to the reference tree).

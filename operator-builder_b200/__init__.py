@@ -1,6 +1,6 @@
-"""operator-builder_b200 -- B200-native marker scanning for operator-builder's `create api` hot path.
+"""operator-builder_b200 -- H100-native marker scanning for operator-builder's `create api` hot path.
 
-Only what the path needs: csrc/ (sm_100a CUDA kernels + the C ABI, built into libobmarkers.so),
+Only what the path needs: csrc/ (sm_90a CUDA kernels + the C ABI, built into libobmarkers.so),
 lexer.py (host mirror of internal/markers/lexer's NewLexer/Run/NextLexeme over GPU tuples),
 go/ (the cgo shim a Go build would compile).  Import as `operator_builder_b200` (the hyphenated
 directory name is what the project brief prescribes; operator_builder_b200.py aliases it).

@@ -46,7 +46,7 @@ def lib():
         return _LIB
     if not os.path.exists(SO_PATH):
         raise ImportError(f"{SO_PATH} is missing: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-                          "(nvcc, sm_100a). operator-builder_b200 has no CPU fallback.")
+                          "(nvcc, sm_90a). operator-builder_b200 has no CPU fallback.")
     L = ctypes.CDLL(SO_PATH)
     vp, u64, u32 = ctypes.c_void_p, ctypes.c_uint64, ctypes.c_uint32
     L.obm_abi_version.restype = ctypes.c_int

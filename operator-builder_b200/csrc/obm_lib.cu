@@ -1,5 +1,5 @@
 /*
- * obm_lib.cu -- libobmarkers.so: CUDA kernels (sm_100a) + the C ABI of include/obmarkers.h.
+ * obm_lib.cu -- libobmarkers.so: CUDA kernels (sm_90a) + the C ABI of include/obmarkers.h.
  *
  * Replaces, for a whole batch of manifests at once, the per-document
  *     lexer.NewLexer(r) ; go l.Run() ; for { l.NextLexeme() }      (internal/markers/lexer/lexer.go:27-53)
@@ -1139,7 +1139,7 @@ extern "C" int obm_marker_index_device(obm_handle *h, const obm_registry *reg, c
 }
 
 /* ---- the same index, FLAT over the tuple stream (the exchange payload of the multi-GPU step) ----------------------------
- * k_marker_index above is a warp per document and spends its time on per-document bookkeeping (1.8 ms per GiB of corpus).
+ * k_marker_index above is a warp per document and spends its time on per-document bookkeeping.
  * Here a thread takes 8 consecutive tuples of the whole stream (four 16-byte loads, coalesced across the warp); the rare
  * MarkerStart candidates (4 % of the tuples) look around through the cache: back for a stale buffer, forward along the
  * Scope / Separator chain (a document's tuples end with EOF or a fatal error, so neither walk leaves the document), then the
@@ -1365,7 +1365,7 @@ extern "C" int obm_marker_index_flat_device(obm_handle *h, const obm_registry *r
 /* ------------------------------------------------------------------------------------------- */
 /* SURVEY.md 8(f) rank 2: collection prefix rewrite (manifests/manifest.go:89-95) on the device  */
 /* SURVEY.md 8(f) rank 4: manifest splitting on "---" lines (manifests/manifest.go:57-80)         */
-/* One warp per document, two passes (count, exclusive scan, write); numbers in profiles/r01_next_rows.json */
+/* One warp per document, two passes (count, exclusive scan, write)                              */
 /* ------------------------------------------------------------------------------------------- */
 __device__ __forceinline__ uint32_t eq_bytes4(uint32_t v, uint32_t pat) { /* 4-bit mask of bytes of v equal to pat's byte (exact for any byte value) */
     const uint32_t t = v ^ pat;

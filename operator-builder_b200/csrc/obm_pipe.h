@@ -10,7 +10,7 @@
  *
  * Why two kernels: in the fused tile kernel (obm_fast.cuh, mode 2) the marker phase is a long dependent chain
  * on a few warps while shared memory caps residency at 3 CTAs/SM and block barriers make every warp wait for
- * the slowest line (profiles/r01_*).  Here K1 has no lexing and K2 has no block barrier.
+ * the slowest line.  Here K1 has no lexing and K2 has no block barrier.
  */
 #ifndef OBM_PIPE_H
 #define OBM_PIPE_H

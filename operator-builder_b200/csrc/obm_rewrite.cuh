@@ -1,7 +1,7 @@
 /*
  * obm_rewrite.cuh -- Manifest.LoadContent's collection rewrite (internal/workload/v1/manifests/manifest.go:89-95) as ONE
  * pass over a packed batch: the text is read once and the rewritten text is written once (2 B of traffic per input byte;
- * r01's kernel read it twice, a warp per document, and moved the runs between deletions byte-interleaved: 3.9 ms per GiB).
+ * r01's kernel read it twice, a warp per document, and moved the runs between deletions byte-interleaved).
  *
  *     ReplaceAll(ReplaceAll(content, "+operator-builder:collection:field", "+operator-builder:field"), "collectionField", "field")
  *

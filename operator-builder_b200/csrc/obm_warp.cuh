@@ -24,8 +24,8 @@
 namespace obmw {
 
 constexpr uint32_t WPC = 10; /* warps per CTA; each works alone on its own shared-memory slice and never meets the others (no barrier).  10 = every
-                              * warp the SM's shared memory holds (23.2 KB each), as ONE CTA: measured 6 % faster than 1-warp CTAs (the CTA's warps are dealt
-                              * round-robin to the four schedulers), profiles/r02_ab_warps_per_cta.txt */
+                              * warp the SM's 227 KB of shared memory holds (23.2 KB each), as ONE CTA so that the CTA's warps are dealt round-robin
+                              * to the SM's four schedulers (single-warp CTAs are not) */
 enum { WC_TICKET = 0 };
 
 __global__ void __launch_bounds__(256)
@@ -133,7 +133,7 @@ __device__ __forceinline__ uint64_t chain_resolve(const WArgs &A, uint32_t u, ui
  * write unit i-1 from W.fin (its exclusive prefix has had a whole unit's time to arrive: no waiting on the chain),
  * assemble unit i into W.fin, scan unit i+1 ...  A unit whose write needs the staged text (documents for the exact
  * lexer, marker lines that are not staged) or that does not fit W.fin is written at once instead. */
-__global__ void __launch_bounds__(WPC * 32, 1) /* one CTA per SM: ptxas may take the registers it wants (153; without the hint it settles for 56 and spills) */
+__global__ void __launch_bounds__(WPC * 32, 1) /* one CTA per SM: ptxas may take the registers it wants (152 on sm_90a; without the hint it settles for fewer and spills) */
 k_warp_scan(WArgs A) {
     extern __shared__ __align__(16) uint8_t smem_raw[];
     WarpSmem &S = reinterpret_cast<WarpSmem *>(smem_raw)[threadIdx.x >> 5];

@@ -24,7 +24,13 @@ def same(got, want):
     return val == want[1]
 
 
-@pytest.mark.parametrize("case", GOLD["cases"], ids=[repr(c["input"])[:40] for c in GOLD["cases"]])
+def case_id(case):
+    """the input's repr, cut to 40 characters; a '::' in it would read as a node-id separator, so its second colon is
+    percent-encoded"""
+    return repr(case["input"])[:40].replace("::", ":%3A")
+
+
+@pytest.mark.parametrize("case", GOLD["cases"], ids=[case_id(c) for c in GOLD["cases"]])
 def test_oracle_reproduces_appendix_d(oracle, case):
     got = oracle.lex(case["input"].encode())
     assert len(got) == len(case["expected"]), (got, case["expected"])

@@ -65,7 +65,7 @@ d_nh = torch.zeros(2, dtype=torch.int32, device=dev)
 ms_hash = timed(lambda: L.obm_hash_batch_device(sc.handle, d_bytes.data_ptr(), d_off.data_ptr(), ndocs, d_out.data_ptr(), d_toff.data_ptr(), d_hash.data_ptr(), d_nh.data_ptr(), st))
 ms_rw = timed(lambda: L.obm_rewrite_collection_markers_device(sc.handle, d_bytes.data_ptr(), d_off.data_ptr(), ndocs, d_rw.data_ptr(), n + 64, d_noff.data_ptr(), st))
 ms_sp = timed(lambda: L.obm_split_docs_device(sc.handle, d_bytes.data_ptr(), d_off.data_ptr(), ndocs, d_rec.data_ptr(), ndocs * 16, d_roff.data_ptr(), st))
-peak = 6583.5
+peak = 3350.0  # H100 SXM data sheet, unless MEASURED_PEAKS.json gives a measured copy peak
 try:
     peak = json.load(open(os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "MEASURED_PEAKS.json")))["hbm_gbs"]
 except Exception:
