@@ -15,7 +15,7 @@ EXPORTS = [
     "obm_pinned_free", "obm_stream_new", "obm_stream_next", "obm_stream_free", "obm_decode_doc", "obm_free", "obm_registry_new", "obm_registry_operator_builder", "obm_registry_add",
     "obm_comm_unique_id", "obm_comm_create", "obm_comm_destroy", "obm_lex_batch_sharded_device",
     "obm_registry_free", "obm_parse_doc", "obm_hash_batch_device", "obm_parse_batch_device", "obm_results_format_doc", "obm_marker_index_device",
-    "obm_marker_index_flat_device", "obm_rewrite_collection_markers_device", "obm_split_docs_device",
+    "obm_marker_index_flat_device", "obm_rewrite_collection_markers_device", "obm_split_docs_device", "obm_lex_collection_batch_device",
 ]
 
 
@@ -83,6 +83,7 @@ def lib():
     L.obm_parse_doc.restype = ctypes.c_int64
     L.obm_rewrite_collection_markers_device.argtypes = [vp, vp, vp, u32, vp, u64, vp, vp]
     L.obm_split_docs_device.argtypes = [vp, vp, vp, u32, vp, u64, vp, vp]
+    L.obm_lex_collection_batch_device.argtypes = [vp, vp, vp, u32, u64, vp, u64, vp, vp, u64, vp, vp, vp, vp]
     L.obm_marker_index_device.argtypes = [vp, vp, vp, vp, u32, vp, vp, vp, u64, vp, vp]
     L.obm_parse_batch_device.argtypes = [vp, vp, vp, vp, u32, u32, vp, vp, vp, u64, vp, u64, vp, vp, vp]
     L.obm_hash_batch_device.argtypes = [vp, vp, vp, u32, vp, vp, vp, vp, vp]

@@ -6,9 +6,11 @@
  *   k_wunit_tiles   unit -> tile
  *   k_warp_scan     persistent warps (no block barrier anywhere): a warp takes a unit by ticket, stages the text of
  *                   each of its units with one TMA bulk copy (cp.async.bulk + mbarrier) into its own slice of shared
- *                   memory and runs obmw::process_unit on it
+ *                   memory and runs obmw::process_unit on it; k_warp_scan<true> also applies the collection rewrite to
+ *                   the staged text and writes the rewritten text out (obm_lex_collection_batch_device)
  */
 #pragma once
+#include <type_traits>
 #include "obm_fast.cuh"
 #include "obm_pipe.cuh"
 
@@ -72,6 +74,10 @@ struct DevHooks {
         if (nbytes) { obmf::mbar_wait(&S.mbar, phase); phase ^= 1u; }
     }
 };
+struct DevHooksRw : DevHooks { /* compute_unit<true>: the rewritten byte count goes on the byte chain right after the compaction */
+    uint64_t *st_bytes, *st_bblocks;
+    __device__ __forceinline__ void publish_bytes(uint32_t u, uint64_t n);
+};
 
 /* ---- the chain over the units' tuple counts ---------------------------------------------------------------
  * Two levels, both fed at PUBLISH time so that nothing on it depends on another warp's (deferred) resolve:
@@ -79,18 +85,19 @@ struct DevHooks {
  *   blk[b]   atomic accumulator of block b = units [32b, 32b+32): count << 56 | sum of tuples
  *   bex[b]   BEX_FLAG | exclusive prefix of block b, stored by whichever unit of the block resolves it first
  * resolve(u) = bex[b] (or a walk back over complete blocks, 32 per step, down to the nearest stored prefix) + the
- * st0 entries of the earlier units of u's own block. */
+ * st0 entries of the earlier units of u's own block.
+ * k_warp_scan<true> runs a second chain of the same shape over the units' rewritten byte counts (A.st_bytes, A.st_bblocks). */
 #define BEX_FLAG (1ull << 63)
-__device__ __forceinline__ void chain_publish(const WArgs &A, uint32_t u, uint64_t total) {
+__device__ __forceinline__ void chain_publish(uint64_t *st_units, uint64_t *st_blocks, uint32_t u, uint64_t total) {
     if ((threadIdx.x & 31) == 0) {
-        reinterpret_cast<volatile uint64_t *>(A.st_tuples)[u] = LB_AGG | total;
-        atomicAdd(reinterpret_cast<unsigned long long *>(A.st_blocks) + (u >> 5), (unsigned long long)((1ull << 56) | total));
+        reinterpret_cast<volatile uint64_t *>(st_units)[u] = LB_AGG | total;
+        atomicAdd(reinterpret_cast<unsigned long long *>(st_blocks) + (u >> 5), (unsigned long long)((1ull << 56) | total));
     }
 }
-__device__ __forceinline__ uint64_t chain_resolve(const WArgs &A, uint32_t u, uint32_t nblocks) {
+__device__ __forceinline__ uint64_t chain_resolve(uint64_t *st_units, uint64_t *st_blocks, uint32_t u, uint32_t nblocks) {
     const uint32_t lane = threadIdx.x & 31;
     const uint32_t b = u >> 5, r = u & 31;
-    volatile uint64_t *st0 = A.st_tuples, *blk = A.st_blocks, *bex = A.st_blocks + nblocks;
+    volatile uint64_t *st0 = st_units, *blk = st_blocks, *bex = st_blocks + nblocks;
     uint64_t s;
     uint32_t backoff = 32; /* ns; doubles up to ~2 us: a thousand warps polling at a fixed short interval saturate L2 and slow the
                             * very warps they wait for (marker-dense units resolve right after publishing) */
@@ -133,6 +140,12 @@ __device__ __forceinline__ uint64_t chain_resolve(const WArgs &A, uint32_t u, ui
  * write unit i-1 from W.fin (its exclusive prefix has had a whole unit's time to arrive: no waiting on the chain),
  * assemble unit i into W.fin, scan unit i+1 ...  A unit whose write needs the staged text (documents for the exact
  * lexer, marker lines that are not staged) or that does not fit W.fin is written at once instead. */
+__device__ __forceinline__ void DevHooksRw::publish_bytes(uint32_t u, uint64_t n) { chain_publish(st_bytes, st_bblocks, u, n); }
+
+/* REWRITE (the collection variant, obm_lex_collection_batch_device): compute_unit compacts the staged text before phase
+ * A and publishes its byte count on the second chain; the rewritten text leaves shared memory (write_text) before the
+ * next unit's bulk copy overwrites it.  k_warp_scan<false> is the plain scan. */
+template <bool REWRITE>
 __global__ void __launch_bounds__(WPC * 32, 1) /* one CTA per SM: ptxas may take the registers it wants (152 on sm_90a; without the hint it settles for fewer and spills) */
 k_warp_scan(WArgs A) {
     extern __shared__ __align__(16) uint8_t smem_raw[];
@@ -143,7 +156,9 @@ k_warp_scan(WArgs A) {
     const obm::Tables T = obmq::dev_tables();
     const uint32_t nunits = (uint32_t)A.ubase[A.ntiles];
     const uint32_t nblocks = (uint32_t)(A.units_max / 32 + 2); /* layout of st_blocks: blk[nblocks] | bex[nblocks] */
-    DevHooks H{0};
+    std::conditional_t<REWRITE, DevHooksRw, DevHooks> H;
+    H.phase = 0;
+    if constexpr (REWRITE) { H.st_bytes = A.st_bytes; H.st_bblocks = A.st_bblocks; }
     WAcc acc{0, 0, 0, 0};
     UnitRegs pend; bool have_pend = false;
     /* unit iterator: UNITS by ticket, in document order (not tiles: a warp that held two units of one tile would publish
@@ -167,17 +182,18 @@ k_warp_scan(WArgs A) {
     while (cur.valid) {
         const UnitDesc nxt = next_unit();
         UnitRegs R;
-        compute_unit(S, S.set, A, T, H, cur, prestaged, R);
-        chain_publish(A, R.u, R.total);
+        compute_unit<REWRITE>(S, S.set, A, T, H, cur, prestaged, R);
+        chain_publish(A.st_tuples, A.st_blocks, R.u, R.total);
+        if constexpr (REWRITE) write_text(S, A, R, chain_resolve(A.st_bytes, A.st_bblocks, R.u, nblocks));
         prestaged = false;
         /* the staged text is dead unless this unit's write needs it: bring in the next unit's text under the assembly and the writes */
         if (!R.needs_text && nxt.valid && nxt.db > nxt.da) { H.stage(S, (const void *)(uintptr_t)nxt.base_abs, desc_load(nxt)); prestaged = true; }
-        if (have_pend) { write_fin(S, A, pend, nunits, chain_resolve(A, pend.u, nblocks)); have_pend = false; }
+        if (have_pend) { write_fin(S, A, pend, nunits, chain_resolve(A.st_tuples, A.st_blocks, pend.u, nblocks)); have_pend = false; }
         if (!R.needs_text && assemble_fin(S, S.set, R, acc)) { pend = R; have_pend = true; }
-        else write_unit(S, S.set, A, T, R, nunits, chain_resolve(A, R.u, nblocks), acc);
+        else write_unit(S, S.set, A, T, R, nunits, chain_resolve(A.st_tuples, A.st_blocks, R.u, nblocks), acc);
         cur = nxt;
     }
-    if (have_pend) write_fin(S, A, pend, nunits, chain_resolve(A, pend.u, nblocks));
+    if (have_pend) write_fin(S, A, pend, nunits, chain_resolve(A.st_tuples, A.st_blocks, pend.u, nblocks));
     uint32_t markers = acc.markers, lexemes = acc.lexemes, exact = acc.exact, fatal = acc.fatal;
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) {

@@ -106,9 +106,11 @@ struct DirectSink {
 #if defined(__CUDA_ARCH__)
 #define OBMW_FFS(x) ((uint32_t)__ffs((int)(x)))
 #define OBMW_FUNNEL_L(lo, hi, s) __funnelshift_l((lo), (hi), (s))
+#define OBMW_FUNNEL_R(lo, hi, s) __funnelshift_r((lo), (hi), (s))
 #else
 #define OBMW_FFS(x) ((uint32_t)__builtin_ffs((int)(x)))
 #define OBMW_FUNNEL_L(lo, hi, s) ((uint32_t)(((((uint64_t)(hi)) << 32) | (uint64_t)(lo)) << ((s) & 31) >> 32))
+#define OBMW_FUNNEL_R(lo, hi, s) ((uint32_t)(((((uint64_t)(hi)) << 32) | (uint64_t)(lo)) >> ((s) & 31)))
 #endif
 
 /* ---- A: byte classes of 32 bytes (8 little-endian words) ------------------------------------------------ */

@@ -171,6 +171,14 @@ class Scanner:
         self._check(self._L.obm_lex_batch_device(self._h, d_bytes, d_doc_off, ndocs, total_bytes, d_out, out_cap,
                                                  d_tuple_off, d_status, d_counts, stream))
 
+    def lex_collection_batch_device(self, d_bytes, d_doc_off, ndocs, total_bytes, d_out_bytes, out_bytes_cap, d_out_doc_off, d_out, out_cap,
+                                    d_tuple_off, d_status=None, d_counts=None, stream=None):
+        """lex_batch_device of a collection batch with Manifest.LoadContent's rewrite fused in (include/obmarkers.h:
+        obm_lex_collection_batch_device): writes the rewritten bytes (d_out_bytes, 16-byte aligned, out_bytes_cap >=
+        total_bytes) and their offsets, and the tuples of the rewritten documents. Asynchronous."""
+        self._check(self._L.obm_lex_collection_batch_device(self._h, d_bytes, d_doc_off, ndocs, total_bytes, d_out_bytes, out_bytes_cap,
+                                                            d_out_doc_off, d_out, out_cap, d_tuple_off, d_status, d_counts, stream))
+
     def parse_batch_device(self, registry, d_bytes, d_doc_off, ndocs, doc_base, d_tuples, d_tuple_off, d_results, res_cap, d_args, arg_cap,
                            d_doc_res_off, d_totals=None, stream=None):
         """The parser on the device (include/obmarkers.h: obm_parse_batch_device). Asynchronous."""
