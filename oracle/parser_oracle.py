@@ -10,6 +10,7 @@ NOT modelled (needs the Go struct types behind marker.Define): Argument.SetValue
 SetArgument is taken to succeed and emit() always succeeds.
 """
 import struct
+from decimal import Decimal
 
 (ERROR, COMMENT, MARKER_START, SCOPE, SEPARATOR, ARG, ARG_ASSIGNMENT, ARG_DELIMITER, STRING, FLOAT, INTEGER, SYNTHETIC_BOOL,
  BOOL, QUOTE) = range(14)
@@ -20,6 +21,49 @@ ZERO = (ERROR, b"", 0, 0)  # receive from the closed channel: lexer.go:51-53
 PARSE_BOOL_TRUE = {b"1", b"t", b"T", b"TRUE", b"true", b"True"}
 PARSE_BOOL_FALSE = {b"0", b"f", b"F", b"FALSE", b"false", b"False"}
 F32_OVERFLOW = 2 ** 128 - 2 ** 103  # smallest magnitude that rounds to +Inf in float32
+F32_OVERFLOW_DEC = Decimal(F32_OVERFLOW)
+
+
+def read_float_magnitude(v: bytes) -> Decimal:
+    """|value| of a decimal literal as strconv's readFloat (atof.go) reads it, exactly: sign, digits with one '.', then
+    an exponent whose digits stop accumulating once it reaches 10000 (so "1e100000" reads as 1e10000).  The digit
+    string goes into a Decimal as it is: no int() (4,300-digit limit) and no float() (inexact, inf)."""
+    i, n = 0, len(v)
+    if i < n and v[i] in b"+-":
+        i += 1
+    digits = bytearray()
+    sawdot, dp = False, 0
+    while i < n:
+        c = v[i]
+        if c == 0x2E:  # '.'
+            if sawdot:
+                break
+            sawdot, dp = True, len(digits)
+        elif 0x30 <= c <= 0x39:
+            if c == 0x30 and not digits:  # leading zeros
+                dp -= 1
+            else:
+                digits.append(c)
+        else:
+            break
+        i += 1
+    if not sawdot:
+        dp = len(digits)
+    if i < n and v[i] in b"eE":
+        i += 1
+        esign = 1
+        if i < n and v[i] in b"+-":
+            esign = -1 if v[i] == 0x2D else 1
+            i += 1
+        e = 0
+        while i < n and 0x30 <= v[i] <= 0x39:
+            if e < 10000:
+                e = e * 10 + v[i] - 0x30
+            i += 1
+        dp += esign * e
+    if not digits:
+        return Decimal(0)
+    return Decimal(f"{digits.decode()}E{dp - len(digits)}")  # 0.d1d2... * 10**dp
 
 
 def go_quote(b: bytes) -> str:
@@ -204,12 +248,7 @@ class Parser:
             self.args.append((arg, "int", self.current[1]))  # the lexer already validated strconv.Atoi (state.go:269)
         elif self.consumed(FLOAT):
             v = self.current[1]
-            try:
-                from fractions import Fraction
-                mag = abs(Fraction(v.decode()))
-            except Exception:  # forms Fraction() does not read ("1.", ".5"): fall back to float()
-                mag = abs(Fraction(float(v.decode())))
-            if mag >= F32_OVERFLOW:
+            if read_float_magnitude(v) >= F32_OVERFLOW_DEC:
                 return self.error(f'strconv.ParseFloat: parsing {go_quote(v)}: value out of range')
             self.args.append((arg, "float", v))
         elif self.consumed(STRING):
