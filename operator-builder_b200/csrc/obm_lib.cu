@@ -470,6 +470,21 @@ extern "C" void obm_destroy(obm_handle *h) {
 /* Number of this library's kernels the last obm_lex_batch_device / obm_lex_batch call launched. */
 extern "C" uint32_t obm_launches_last_call(const obm_handle *h) { return h ? h->launches : 0; }
 
+#ifdef OBMW_PHASE_CLOCKS
+/* the phase-clock build only: k_warp_scan's cycles per bucket (obmw::PC_*, summed over warps) and, at [PC_N], the units,
+ * accumulated over every launch on the current device since the last reset; reset != 0 zeroes them after the read */
+extern "C" int obm_phase_cycles(unsigned long long *out, int reset) {
+    if (cudaDeviceSynchronize() != cudaSuccess) return OBM_E_CUDA;
+    if (out && cudaMemcpyFromSymbol(out, obmw::g_phase_cycles, sizeof(obmw::g_phase_cycles)) != cudaSuccess) return OBM_E_CUDA;
+    if (reset) {
+        const unsigned long long z[obmw::PC_N + 1] = {};
+        if (cudaMemcpyToSymbol(obmw::g_phase_cycles, z, sizeof(z)) != cudaSuccess) return OBM_E_CUDA;
+    }
+    return OBM_OK;
+}
+extern "C" int obm_phase_buckets(void) { return (int)obmw::PC_N; }
+#endif
+
 /* Chunk size of the overlapped host path (obm_lex_batch pipelines batches of >= 2 chunks). Returns the old value. */
 extern "C" uint64_t obm_set_chunk_bytes(obm_handle *h, uint64_t bytes) { uint64_t old = h->chunk_bytes; if (bytes >= 4096) h->chunk_bytes = bytes; return old; }
 

@@ -29,6 +29,9 @@ constexpr uint32_t WPC = 10; /* warps per CTA; each works alone on its own share
                               * warp the SM's 227 KB of shared memory holds (23.2 KB each), as ONE CTA so that the CTA's warps are dealt round-robin
                               * to the SM's four schedulers (single-warp CTAs are not) */
 enum { WC_TICKET = 0 };
+#ifdef OBMW_PHASE_CLOCKS
+__device__ unsigned long long g_phase_cycles[PC_N + 1]; /* cycles per bucket summed over warps; [PC_N]: units */
+#endif
 
 __global__ void __launch_bounds__(256)
 k_wtile_index(const uint64_t *__restrict__ doc_off, uint32_t ndocs, uint32_t ntiles, uint32_t *__restrict__ tile_first,
@@ -146,7 +149,7 @@ __device__ __forceinline__ void DevHooksRw::publish_bytes(uint32_t u, uint64_t n
  * A and publishes its byte count on the second chain; the rewritten text leaves shared memory (write_text) before the
  * next unit's bulk copy overwrites it.  k_warp_scan<false> is the plain scan. */
 template <bool REWRITE>
-__global__ void __launch_bounds__(WPC * 32, 1) /* one CTA per SM: ptxas may take the registers it wants (152 on sm_90a; without the hint it settles for fewer and spills) */
+__global__ void __launch_bounds__(WPC * 32, 1) /* one CTA per SM: ptxas may take the registers it wants (151 on sm_90a; without the hint it settles for fewer and spills) */
 k_warp_scan(WArgs A) {
     extern __shared__ __align__(16) uint8_t smem_raw[];
     WarpSmem &S = reinterpret_cast<WarpSmem *>(smem_raw)[threadIdx.x >> 5];
@@ -177,23 +180,57 @@ k_warp_scan(WArgs A) {
         return make_desc(A, u, da, db, extra);
     };
     if (lane == 0) tn = atomicAdd(&A.ctl[WC_TICKET], 1u);
+#ifdef OBMW_PHASE_CLOCKS
+    PhaseClk pc{};
+    pc.t0 = (uint32_t)clock64();
+    uint32_t pc_units = 0;
+#endif
     UnitDesc cur = next_unit();
     bool prestaged = false;
     while (cur.valid) {
         const UnitDesc nxt = next_unit();
+        OBMW_PC_MARK(PC_OTHER);
         UnitRegs R;
-        compute_unit<REWRITE>(S, S.set, A, T, H, cur, prestaged, R);
+        compute_unit<REWRITE>(S, S.set, A, T, H, cur, prestaged, R OBMW_PC_ARG);
         chain_publish(A.st_tuples, A.st_blocks, R.u, R.total);
         if constexpr (REWRITE) write_text(S, A, R, chain_resolve(A.st_bytes, A.st_bblocks, R.u, nblocks));
         prestaged = false;
         /* the staged text is dead unless this unit's write needs it: bring in the next unit's text under the assembly and the writes */
         if (!R.needs_text && nxt.valid && nxt.db > nxt.da) { H.stage(S, (const void *)(uintptr_t)nxt.base_abs, desc_load(nxt)); prestaged = true; }
-        if (have_pend) { write_fin(S, A, pend, nunits, chain_resolve(A.st_tuples, A.st_blocks, pend.u, nblocks)); have_pend = false; }
-        if (!R.needs_text && assemble_fin(S, S.set, R, acc)) { pend = R; have_pend = true; }
-        else write_unit(S, S.set, A, T, R, nunits, chain_resolve(A.st_tuples, A.st_blocks, R.u, nblocks), acc);
+        OBMW_PC_MARK(PC_OTHER);
+        if (have_pend) {
+            const uint64_t base = chain_resolve(A.st_tuples, A.st_blocks, pend.u, nblocks);
+            OBMW_PC_MARK(PC_CHAIN);
+            write_fin(S, A, pend, nunits, base);
+            OBMW_PC_MARK(PC_WRITE);
+            have_pend = false;
+        }
+        if (!R.needs_text && assemble_fin(S, S.set, R, acc)) { pend = R; have_pend = true; OBMW_PC_MARK(PC_AFIN); }
+        else {
+            OBMW_PC_MARK(PC_AFIN);
+            const uint64_t base = chain_resolve(A.st_tuples, A.st_blocks, R.u, nblocks);
+            OBMW_PC_MARK(PC_CHAIN);
+            write_unit(S, S.set, A, T, R, nunits, base, acc OBMW_PC_ARG);
+            OBMW_PC_MARK(PC_WRITE);
+        }
         cur = nxt;
+#ifdef OBMW_PHASE_CLOCKS
+        pc_units++;
+#endif
     }
-    if (have_pend) write_fin(S, A, pend, nunits, chain_resolve(A.st_tuples, A.st_blocks, pend.u, nblocks));
+    if (have_pend) {
+        const uint64_t base = chain_resolve(A.st_tuples, A.st_blocks, pend.u, nblocks);
+        OBMW_PC_MARK(PC_CHAIN);
+        write_fin(S, A, pend, nunits, base);
+        OBMW_PC_MARK(PC_WRITE);
+    }
+#ifdef OBMW_PHASE_CLOCKS
+    if (lane == 0) {
+#pragma unroll
+        for (uint32_t b = 0; b < PC_N; b++) atomicAdd(&g_phase_cycles[b], (unsigned long long)pc.c[b]);
+        atomicAdd(&g_phase_cycles[PC_N], (unsigned long long)pc_units);
+    }
+#endif
     uint32_t markers = acc.markers, lexemes = acc.lexemes, exact = acc.exact, fatal = acc.fatal;
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) {

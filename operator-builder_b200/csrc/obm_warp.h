@@ -6,7 +6,7 @@
  * copy, obm_warp.cuh) and everything else happens inside the warp, without a block barrier and without a
  * second read of the text from HBM:
  *
- *   A  rows      1 KiB per step, 32 bytes per lane: SIMD-within-register byte classes -> newline / special
+ *   A  steps     2 KiB per step, 64 contiguous bytes per lane: SIMD-within-register byte classes -> newline / special
  *                bitmaps ('#', '+', "//": what can start a comment or a marker in lex / lexComment,
  *                state.go:20-33,48), bit-parallel "first special of every line" ((~events + starts) & events with
  *                a ballot carry look-ahead across lanes), newline prefix counts -> owner list in position order
@@ -42,7 +42,8 @@ namespace obmw {
 constexpr uint32_t TILE = OBMW_TILE;      /* a unit = the documents starting in [t*TILE, (t+1)*TILE) (split when > DMAX / > BUFB) */
 constexpr uint32_t BUFB = OBMW_BUFB;      /* bytes of text staged per warp */
 constexpr uint32_t MAXDOC = (BUFB - 16 < 16368u) ? BUFB - 16 : 16368u; /* larger documents take the chunk-parallel exact path */
-constexpr uint32_t ROW = 1024;            /* bytes per row step: 32 per lane */
+constexpr uint32_t ROW = 1024;            /* bytes per bitmap row: 32 words, one W.naw entry (rewrite_staged steps by rows, 32 bytes per lane) */
+constexpr uint32_t STEP = 2048;           /* bytes per phase-A step: 64 per lane, words 2L and 2L+1 (one W.nlpre entry) */
 constexpr uint32_t NWORDS = BUFB / 32;    /* 32-byte words of the bitmaps */
 constexpr uint32_t DMAX = 31;             /* documents per unit: one lane each, lane nd holds the end */
 constexpr uint32_t OWN_CAP = 256;         /* owning lines per unit (more: the unit is paged, document by document; a document with more: the exact lexer) */
@@ -105,10 +106,14 @@ struct DirectSink {
 
 #if defined(__CUDA_ARCH__)
 #define OBMW_FFS(x) ((uint32_t)__ffs((int)(x)))
+#define OBMW_FFS64(x) ((uint32_t)__ffsll((long long)(x)))
+#define OBMW_POPC64(x) ((uint32_t)__popcll(x))
 #define OBMW_FUNNEL_L(lo, hi, s) __funnelshift_l((lo), (hi), (s))
 #define OBMW_FUNNEL_R(lo, hi, s) __funnelshift_r((lo), (hi), (s))
 #else
 #define OBMW_FFS(x) ((uint32_t)__builtin_ffs((int)(x)))
+#define OBMW_FFS64(x) ((uint32_t)__builtin_ffsll((long long)(x)))
+#define OBMW_POPC64(x) ((uint32_t)__builtin_popcountll(x))
 #define OBMW_FUNNEL_L(lo, hi, s) ((uint32_t)(((((uint64_t)(hi)) << 32) | (uint64_t)(lo)) << ((s) & 31) >> 32))
 #define OBMW_FUNNEL_R(lo, hi, s) ((uint32_t)(((((uint64_t)(hi)) << 32) | (uint64_t)(lo)) >> ((s) & 31)))
 #endif
@@ -146,6 +151,20 @@ OBM_HD uint32_t range_mask(uint32_t pos0, uint32_t lo, uint32_t hi) {
     if (lo > pos0) keep &= (lo - pos0 >= 32u) ? 0u : (0xFFFFFFFFu << (lo - pos0));
     if (hi < pos0 + 32u) keep &= (hi <= pos0) ? 0u : (0xFFFFFFFFu >> (pos0 + 32u - hi));
     return keep;
+}
+/* bits of [pos0, pos0+64) that lie inside [lo, hi) */
+OBM_HD uint64_t range_mask64(uint32_t pos0, uint32_t lo, uint32_t hi) {
+    uint64_t keep = ~0ull;
+    if (lo > pos0) keep &= (lo - pos0 >= 64u) ? 0ull : (~0ull << (lo - pos0));
+    if (hi < pos0 + 64u) keep &= (hi <= pos0) ? 0ull : (~0ull >> (pos0 + 64u - hi));
+    return keep;
+}
+/* bits 0..15 of v to the even bits 0, 2, .., 30 */
+OBM_HD uint32_t spread16(uint32_t v) {
+    v &= 0xFFFFu;
+    v = (v | (v << 8)) & 0x00FF00FFu; v = (v | (v << 4)) & 0x0F0F0F0Fu;
+    v = (v | (v << 2)) & 0x33333333u; v = (v | (v << 1)) & 0x55555555u;
+    return v;
 }
 
 /* ---- C: the stepper ------------------------------------------------------------------------------------

@@ -35,6 +35,21 @@
 
 namespace obmw {
 
+/* ---- OBMW_PHASE_CLOCKS (a separate device build, libobmarkers_phase.so): k_warp_scan adds the cycles between phase
+ * borders into per-warp registers and sums them over the warps at kernel end (tools/phase_cycles.py).  Off, the
+ * macros below are empty and the kernels compile as without them. ---- */
+enum : uint32_t { PC_STAGE, PC_A, PC_B, PC_C, PC_ASM, PC_AFIN, PC_WRITE, PC_CHAIN, PC_OTHER, PC_N };
+#if defined(OBMW_PHASE_CLOCKS) && defined(__CUDACC__)
+struct PhaseClk { uint32_t t0; uint32_t c[PC_N]; }; /* low 32 bits of clock64(): a warp's share of one launch stays far below 2^32 cycles */
+#define OBMW_PC_PARAM , PhaseClk &pc
+#define OBMW_PC_ARG , pc
+#define OBMW_PC_MARK(b) do { const uint32_t t_ = (uint32_t)clock64(); pc.c[(b)] += t_ - pc.t0; pc.t0 = t_; } while (0)
+#else
+#define OBMW_PC_PARAM
+#define OBMW_PC_ARG
+#define OBMW_PC_MARK(b) ((void)0)
+#endif
+
 /* scratch of the unit being scanned */
 struct UnitSet {
     union {
@@ -61,6 +76,7 @@ struct WarpSmem {
 };
 static_assert(sizeof(uint32_t) * MLCAP * LTS <= sizeof(uint32_t) * 2 * NWORDS, "the staging area overlays the bitmaps");
 static_assert(OWN_CAP <= 256, "mlist holds owner indices in a byte");
+static_assert(STEP == 64 * 32 && STEP == 2 * ROW && (BUFB + STEP - 1) / STEP * 2 <= NWORDS / 32 + 1, "phase A writes both naw rows of its last step");
 
 /* a scanned unit between its two halves: warp-uniform values, and one document per lane */
 struct UnitRegs {
@@ -195,7 +211,7 @@ OBM_FN bool utf8_plain_w(const WarpSmem &W, uint32_t q, uint32_t e) {
  * [lo_pos, hi_pos) and whose starts / flags are in W.dstart[0..nd] / W.dflag[0..nd).  Returns false (nothing assembled)
  * when the range has more owning lines than OWN_CAP and the caller can split it (allow_page). ---- */
 OBMW_DEV bool scan_range(WarpSmem &W, UnitSet &S, const WArgs &A, const obm::Tables &T, uint32_t u, uint32_t da, uint32_t nd,
-                         uint32_t lo_pos, uint32_t hi_pos, bool allow_page, UnitRegs &R) {
+                         uint32_t lo_pos, uint32_t hi_pos, bool allow_page, UnitRegs &R OBMW_PC_PARAM) {
     (void)A;
     const uint32_t lane = WLANE();
     uint32_t n_owners = 0, n_ml = 0;
@@ -203,75 +219,99 @@ OBMW_DEV bool scan_range(WarpSmem &W, UnitSet &S, const WArgs &A, const obm::Tab
     if (nd) {
         const auto text = WTEXT(W);
 
-        /* ---- A: rows ---- */
-        const uint32_t r0 = lo_pos / ROW, r1 = (hi_pos + ROW - 1) / ROW;
-        uint32_t nl_run = 0, own_run = 0, cin_row = 0, prev_top = 0, nextd = 1;
-        for (uint32_t r = r0; r < r1; r++) {
-            const uint32_t row0 = r * ROW, pos0 = row0 + lane * 32u;
-            uint32_t x[8];
-            {
-                const uint4 a = reinterpret_cast<const uint4 *>(W.text + pos0)[0], b = reinterpret_cast<const uint4 *>(W.text + pos0)[1];
-                x[0] = a.x; x[1] = a.y; x[2] = a.z; x[3] = a.w; x[4] = b.x; x[5] = b.y; x[6] = b.z; x[7] = b.w;
+        /* ---- A: steps of STEP bytes; lane L owns the 64 contiguous bytes [pos0, pos0 + 64) = bitmap words 2L, 2L+1 of the
+         * step.  A lane whose bytes lie wholly at or past hi_pos neither loads nor stores: the last step can reach past
+         * the staged text, the bitmaps and W.nlpre (nothing reads the words past hi_pos) ---- */
+        const uint32_t s0 = lo_pos / STEP, s1 = (hi_pos + STEP - 1) / STEP;
+        uint32_t nl_run = 0, own_run = 0, cin_step = 0, prev_top = 0, nextd = 1;
+        for (uint32_t s = s0; s < s1; s++) {
+            const uint32_t step0 = s * STEP, pos0 = step0 + lane * 64u;
+            const bool live = pos0 < hi_pos;
+            uint32_t xa[8] = {0, 0, 0, 0, 0, 0, 0, 0}, xb[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+            if (live) {
+                const uint4 *q4 = reinterpret_cast<const uint4 *>(W.text + pos0);
+                const uint4 a = q4[0], b = q4[1], c = q4[2], d = q4[3];
+                xa[0] = a.x; xa[1] = a.y; xa[2] = a.z; xa[3] = a.w; xa[4] = b.x; xa[5] = b.y; xa[6] = b.z; xa[7] = b.w;
+                xb[0] = c.x; xb[1] = c.y; xb[2] = c.z; xb[3] = c.w; xb[4] = d.x; xb[5] = d.y; xb[6] = d.z; xb[7] = d.w;
             }
-            const Masks m = classify32(x);
-            const uint32_t keep = range_mask(pos0, lo_pos, hi_pos);
-            uint32_t nl = m.nl & keep;
-            const uint32_t hp = m.hp & keep, sl = m.sl & keep;
-            /* bytes >= 0x80 inside the range: the documents that hold them take the exact lexer */
-            bool na = false;
-            if (m.hi && keep) {
-                if (keep == 0xFFFFFFFFu) na = true;
-                else for (uint32_t k = 0; k < 32; k++) if (((keep >> k) & 1u) && W.text[pos0 + k] >= 0x80) na = true;
-            }
-            const uint32_t nab = WBALLOT(na);
-            if (lane == 0) W.naw[r] = nab;
-            if (nab && lane < nd) { /* rare: exact attribution, byte by byte */
-                const uint32_t q = W.dstart[lane], e = W.dstart[lane + 1];
-                for (uint32_t mm = nab; mm; mm &= mm - 1) {
-                    const uint32_t l0 = row0 + (OBMW_FFS(mm) - 1u) * 32u;
-                    const uint32_t a = q > l0 ? q : l0, b = e < l0 + 32u ? e : l0 + 32u;
-                    for (uint32_t p = a; p < b; p++) if (W.text[p] >= 0x80) W.dflag[lane] |= DF_NONASCII;
+            const uint64_t keep = range_mask64(pos0, lo_pos, hi_pos);
+            Masks ma = classify32_t<false>(xa), mb = classify32_t<false>(xb);
+            bool na0 = false, na1 = false; /* bytes >= 0x80 inside the range, per 32-byte word: their documents take the exact lexer */
+            if (ma.hi | mb.hi) { /* rare; kept out of line (one copy of the exact classifier, one byte loop) to keep the hot loop small */
+#pragma unroll 1
+                for (uint32_t h = 0; h < 2; h++) { /* the carry-free byte test is only exact for 7-bit input */
+                    uint32_t x[8];
+#pragma unroll
+                    for (int k = 0; k < 8; k++) x[k] = h ? xb[k] : xa[k];
+                    Masks m = classify32_t<true>(x);
+                    if (h) { m.hi = mb.hi; mb = m; } else { m.hi = ma.hi; ma = m; }
+                }
+                if (keep == ~0ull) { na0 = ma.hi != 0; na1 = mb.hi != 0; }
+                else {
+#pragma unroll 1
+                    for (uint32_t k = 0; k < 64; k++) if (((keep >> k) & 1u) && W.text[pos0 + k] >= 0x80) { if (k < 32) na0 = true; else na1 = true; }
                 }
             }
-            /* "//": a '/' whose successor is a '/' (the successor of the lane's last byte sits in the next lane's chunk) */
-            const uint32_t nxt = (pos0 + 32u < hi_pos && W.text[pos0 + 32u] == '/') ? 0x80000000u : 0u;
-            uint32_t ss = sl & ((sl >> 1) | nxt);
+            uint64_t nl = ((uint64_t)ma.nl | ((uint64_t)mb.nl << 32)) & keep;
+            const uint64_t hp = ((uint64_t)ma.hp | ((uint64_t)mb.hp << 32)) & keep, sl = ((uint64_t)ma.sl | ((uint64_t)mb.sl << 32)) & keep;
+            const uint32_t nae = WBALLOT(na0), nao = WBALLOT(na1); /* even / odd words of the step */
+            if (nae | nao) { /* rare: the two rows' W.naw entries interleave the ballots; exact attribution, byte by byte */
+                const uint32_t w0 = spread16(nae) | (spread16(nao) << 1), w1 = spread16(nae >> 16) | (spread16(nao >> 16) << 1);
+                if (lane == 0) { W.naw[2u * s] = w0; W.naw[2u * s + 1u] = w1; }
+                if (lane < nd) {
+                    const uint32_t q = W.dstart[lane], e = W.dstart[lane + 1];
+                    for (uint32_t h = 0; h < 2; h++) {
+                        for (uint32_t mm = h ? w1 : w0; mm; mm &= mm - 1) {
+                            const uint32_t l0 = step0 + h * ROW + (OBMW_FFS(mm) - 1u) * 32u;
+                            const uint32_t a = q > l0 ? q : l0, b = e < l0 + 32u ? e : l0 + 32u;
+                            for (uint32_t p = a; p < b; p++) if (W.text[p] >= 0x80) W.dflag[lane] |= DF_NONASCII;
+                        }
+                    }
+                }
+            } else if (lane == 0) { W.naw[2u * s] = 0; W.naw[2u * s + 1u] = 0; }
+            /* "//": a '/' whose successor is a '/' (the successor of the lane's last byte sits in the next lane's bytes) */
+            const uint64_t nxt = (pos0 + 64u < hi_pos && W.text[pos0 + 64u] == '/') ? (1ull << 63) : 0ull;
+            uint64_t ss = sl & ((sl >> 1) | nxt);
             /* virtual newline on the byte before every document start (a line starts there, whatever the byte is) */
             while (nextd < nd) {
                 const uint32_t q = W.dstart[nextd];
                 if (q > lo_pos) {
-                    if (q - 1u >= row0 + ROW) break;
-                    if (((q - 1u - row0) >> 5) == lane) { const uint32_t bit = 1u << ((q - 1u) & 31u); nl |= bit; ss &= ~bit; }
+                    if (q - 1u >= step0 + STEP) break;
+                    if (((q - 1u - step0) >> 6) == lane) { const uint64_t bit = 1ull << ((q - 1u) & 63u); nl |= bit; ss &= ~bit; }
                 }
                 nextd++;
             }
-            const uint32_t sp = hp | ss;
-            const uint32_t ev = nl | sp;
+            const uint64_t sp = hp | ss;
+            const uint64_t ev = nl | sp;
             /* line starts: after every newline, and at the first byte of the range */
-            const uint32_t top = nl >> 31;
+            const uint32_t top = (uint32_t)(nl >> 63);
             uint32_t up = WSHFL_UP(top, 1);
             if (lane == 0) up = prev_top;
-            uint32_t M = (nl << 1) | up;
-            if (r == r0 && lo_pos < hi_pos && ((lo_pos - row0) >> 5) == lane) M |= 1u << (lo_pos & 31u);
+            uint64_t M = (nl << 1) | up;
+            if (s == s0 && lo_pos < hi_pos && ((lo_pos - step0) >> 6) == lane) M |= 1ull << (lo_pos & 63u);
             /* first event of every line: (~ev + M) & ev, the carry resolved across lanes by generate / propagate */
-            const uint32_t G = (uint32_t)((((uint64_t)(~ev)) + M) >> 32);
-            const uint32_t Gb = WBALLOT(G != 0), Pb = WBALLOT(ev == 0 && G == 0);
+            const uint64_t nev = ~ev, sum = nev + M;
+            const bool G = sum < nev; /* carry out of the lane's 64 bits */
+            const uint32_t Gb = WBALLOT(G), Pb = WBALLOT(ev == 0 && !G);
             uint32_t cout;
-            const uint32_t Cm = obmt::carry_lookahead32(Gb, Pb, cin_row, &cout);
+            const uint32_t Cm = obmt::carry_lookahead32(Gb, Pb, cin_step, &cout);
             const uint32_t cin = (Cm >> lane) & 1u;
-            uint32_t own = (uint32_t)(((uint64_t)(~ev)) + M + cin) & ev & sp;
-            cin_row = cout;
+            uint64_t own = (sum + cin) & ev & sp;
+            cin_step = cout;
             prev_top = WSHFL(top, 31);
-            S.u.bm.nlw[r * 32u + lane] = nl;
-            S.u.bm.spw[r * 32u + lane] = sp;
-            uint32_t cnt = OBMT_POPC(nl) | (OBMT_POPC(own) << 16);
+            const uint32_t wi = 2u * (s * 32u + lane);
+            if (live) {
+                S.u.bm.nlw[wi] = (uint32_t)nl; S.u.bm.nlw[wi + 1u] = (uint32_t)(nl >> 32);
+                S.u.bm.spw[wi] = (uint32_t)sp; S.u.bm.spw[wi + 1u] = (uint32_t)(sp >> 32);
+            }
+            uint32_t cnt = OBMW_POPC64(nl) | (OBMW_POPC64(own) << 16); /* a step holds at most 2,048 of either */
             const uint32_t mine = cnt;
             OBMW_SCAN_INCL(cnt);
             const uint32_t excl = cnt - mine;
-            if (!(lane & 1u)) W.nlpre[r * 16u + (lane >> 1)] = (uint16_t)(nl_run + (excl & 0xFFFFu));
+            if (live) W.nlpre[s * 32u + lane] = (uint16_t)(nl_run + (excl & 0xFFFFu));
             uint32_t o = own_run + (excl >> 16);
             while (own) {
-                if (o < OWN_CAP) S.orec[o] = pos0 + (OBMW_FFS(own) - 1u);
+                if (o < OWN_CAP) S.orec[o] = pos0 + (OBMW_FFS64(own) - 1u);
                 o++; own &= own - 1u;
             }
             const uint32_t tot = WSHFL(cnt, 31);
@@ -285,6 +325,7 @@ OBMW_DEV bool scan_range(WarpSmem &W, UnitSet &S, const WArgs &A, const obm::Tab
         }
         if (lane < nd && W.dflag[lane] == DF_NONASCII && utf8_plain_w(W, W.dstart[lane], W.dstart[lane + 1])) W.dflag[lane] = DF_UNI;
         WSYNC();
+        OBMW_PC_MARK(PC_A);
 
         /* ---- B: owners ---- */
         for (uint32_t o0 = 0; o0 < n_owners; o0 += 32) {
@@ -336,6 +377,7 @@ OBMW_DEV bool scan_range(WarpSmem &W, UnitSet &S, const WArgs &A, const obm::Tab
 
         if (lane < nd) W.dflag[lane] &= ~DF_UNI; /* from here on a set flag means: the exact lexer */
         WSYNC();
+        OBMW_PC_MARK(PC_B);
         /* ---- C: marker lines, a lane per line; the first MLCAP lines stage their tuples ---- */
         for (uint32_t k0 = 0; k0 < n_ml; k0 += 32) {
             const uint32_t k = k0 + lane; const bool on = k < n_ml;
@@ -365,6 +407,7 @@ OBMW_DEV bool scan_range(WarpSmem &W, UnitSet &S, const WArgs &A, const obm::Tab
             }
         }
         WSYNC();
+        OBMW_PC_MARK(PC_C);
     }
 
     /* ---- assembly: counts -> positions inside the unit ---- */
@@ -420,6 +463,7 @@ OBMW_DEV bool scan_range(WarpSmem &W, UnitSet &S, const WArgs &A, const obm::Tab
     R.dflag = dflag; R.dtot = dtot; R.dexcl = dexcl; R.dlen = dlen;
     R.needs_text = WBALLOT(unstaged || dflag != 0) != 0;
     R.paged = false;
+    OBMW_PC_MARK(PC_ASM);
     return true;
 }
 
@@ -517,7 +561,7 @@ OBMW_DEV uint32_t rewrite_staged(WarpSmem &W, UnitSet &S, uint32_t nd, uint32_t 
 
 /* ---- first half of a unit: stage its text, scan it, assemble the tuple positions ---- */
 template <bool REWRITE = false, class Hooks>
-OBMW_DEV void compute_unit(WarpSmem &W, UnitSet &S, const WArgs &A, const obm::Tables &T, Hooks &H, const UnitDesc &D, bool prestaged, UnitRegs &R) {
+OBMW_DEV void compute_unit(WarpSmem &W, UnitSet &S, const WArgs &A, const obm::Tables &T, Hooks &H, const UnitDesc &D, bool prestaged, UnitRegs &R OBMW_PC_PARAM) {
     const uint32_t lane = WLANE();
     const uint32_t u = D.u, da = D.da, nd = D.db - D.da, extra = D.extra;
     uint32_t lo_pos = 0, hi_pos = 0;
@@ -530,6 +574,7 @@ OBMW_DEV void compute_unit(WarpSmem &W, UnitSet &S, const WArgs &A, const obm::T
         if (lane < nd) W.dflag[lane] = 0;
         WSYNC();
         H.stage_wait(W, load);
+        OBMW_PC_MARK(PC_STAGE); /* the rewrite of k_warp_scan<true> counts as phase A */
         if constexpr (REWRITE) hi_pos = rewrite_staged(W, S, nd, lo_pos, hi_pos);
     }
     uint64_t nbytes = 0;
@@ -548,7 +593,7 @@ OBMW_DEV void compute_unit(WarpSmem &W, UnitSet &S, const WArgs &A, const obm::T
             if (lane == 0) { W.dstart[0] = pj; W.dstart[1] = ej; W.dflag[0] = 0; }
             WSYNC();
         }
-        const bool ok = scan_range(W, S, A, T, u, whole ? da : da + j, whole ? nd : 1u, pj, ej, whole && nd > 1, R);
+        const bool ok = scan_range(W, S, A, T, u, whole ? da : da + j, whole ? nd : 1u, pj, ej, whole && nd > 1, R OBMW_PC_ARG);
         if (whole) {
             if (ok) break;
             mypos = lane <= nd ? W.dstart[lane] : 0u;
@@ -668,7 +713,8 @@ OBMW_DEV void write_fin(const WarpSmem &W, const WArgs &A, const UnitRegs &R, ui
 /* ---- second half: the unit's tuples at their final positions (base = tuples of all earlier units) ----------
  * The direct path: units with needs_text, or too large for W.fin; written before the warp stages its next unit. */
 OBMW_DEV void write_range(WarpSmem &W, UnitSet &S, const WArgs &A, const obm::Tables &T, const UnitRegs &R, uint64_t base, WAcc &acc);
-OBMW_DEV void write_unit(WarpSmem &W, UnitSet &S, const WArgs &A, const obm::Tables &T, const UnitRegs &R, uint32_t nunits, uint64_t base, WAcc &acc) {
+OBMW_DEV void write_unit(WarpSmem &W, UnitSet &S, const WArgs &A, const obm::Tables &T, const UnitRegs &R, uint32_t nunits, uint64_t base, WAcc &acc
+                         OBMW_PC_PARAM) {
     const uint32_t lane = WLANE();
     if (lane == 0) {
         if (R.u == 0) A.tuple_off[0] = 0;
@@ -687,9 +733,10 @@ OBMW_DEV void write_unit(WarpSmem &W, UnitSet &S, const WArgs &A, const obm::Tab
             bj = base + WSHFL(R.dexcl, j);
             if (lane == 0) { W.dstart[0] = pj; W.dstart[1] = ej; W.dflag[0] = 0; }
             WSYNC();
-            scan_range(W, S, A, T, R.u, R.da + j, 1, pj, ej, false, Rj);
+            scan_range(W, S, A, T, R.u, R.da + j, 1, pj, ej, false, Rj OBMW_PC_ARG);
         }
         write_range(W, S, A, T, Rj, bj, acc);
+        OBMW_PC_MARK(PC_WRITE);
     }
 }
 /* the documents of a scanned range: tuples at their final positions (base = tuples before the range's first document) */
