@@ -272,11 +272,22 @@ void obm_free(void *p);
  * (state.go:13-175, definition.go:13-21, emit.go:8-24, error.go:8-22) over obm_stream_*.  A registry lists the
  * marker names (with their leading '+', e.g. "+operator-builder:field") and the argument names each accepts
  * (marker/marker.go LookupArgument).  obm_parse_doc returns the number of Results and a malloc'd record
- * buffer (format: csrc/obm_parse.cpp); Argument.SetValue / InflateObject type checks are not modelled.
+ * buffer (format: csrc/obm_parse.cpp).
+ * A definition added with names only (obm_registry_add, obm_registry_operator_builder) accepts every value: each
+ * SetArgument succeeds and emit() always succeeds.  A definition added by obm_registry_define carries the Go types of
+ * marker.Define(name, T{}) and gets the reference's SetArgument (marker/argument.go:91-127: wrong type, the FieldType
+ * unmarshal error, the int -> string reflect.Set panic) and InflateObject (marker/marker.go:65-95: missing required
+ * arguments).  Parity unpinned: the reference has no parser tests; only the FieldType names are pinned
+ * (field_types_internal_test.go).  Go lists missing arguments in map order; here they are in definition order.
  */
 obm_registry *obm_registry_new(void);
-obm_registry *obm_registry_operator_builder(void); /* field / collection:field / resource markers */
+obm_registry *obm_registry_operator_builder(void); /* field / collection:field / resource markers, names only */
 int obm_registry_add(obm_registry *r, const char *marker_name, const char *const *arg_names, uint32_t nargs);
+/* internal/workload/v1/markers/markers.go:20-25 (MarkerType) and :92-113 (the definition each adds) */
+enum { OBM_FIELD_MARKER = 0, OBM_COLLECTION_MARKER = 1, OBM_RESOURCE_MARKER = 2 };
+/* Adds the typed definition of one marker type; defining a name again replaces it (Registry.Add, marker/registry.go:20-22).
+ * Build InspectForYAML's subsets this way, e.g. resource only (child_resource.go:71).  OBM_E_ARG for another type. */
+int obm_registry_define(obm_registry *r, int marker_type);
 void obm_registry_free(obm_registry *r);
 /*
  * Device side of the same row: a compact index of the REGISTERED markers in a tuple stream that is still in
@@ -315,21 +326,32 @@ typedef struct obm_result {
     uint32_t text_off;   /* MarkerText = doc[text_off, text_off + text_len) (+ "\n" when OBM_R_NL) */
     uint32_t text_len;
     uint16_t reg_id;     /* registry entry; 0xFFFF on OBM_R_HOST records */
-    uint16_t nargs;      /* error results: 1 = {name_off: line, val_off/val_len: the offending literal} */
+    uint16_t nargs;      /* error results: 1 = {name_off: line, val_off/val_len: the offending literal}; OBM_R_ERR_MISSING: 0 */
     uint32_t arg_base;   /* index of the first obm_arg of this result in the batch's argument array */
     uint32_t flags;      /* OBM_R_* */
-    uint32_t aux;        /* error results: column of parser.current; OBM_R_HOST: the first unmodelled tuple kind */
+    uint32_t aux;        /* error results: column of parser.current; OBM_R_HOST: the first unmodelled tuple kind;
+                            OBM_R_ERR_MISSING: bit j = the definition's argument j is required and was never set */
 } obm_result;
 typedef struct obm_arg {
     uint32_t name_off;   /* argument name = doc[name_off, name_off + name_len) */
     uint32_t val_off;    /* value = doc[val_off, val_off + val_len); OBM_A_SYNTHETIC_TRUE: the value is "true" */
     uint32_t val_len;
-    uint16_t name_len;
+    uint16_t name_len;   /* OBM_R_ERR_SETARG / OBM_R_PANIC: the argument's index in its definition (name_off: line) */
     uint8_t kind;        /* 0 bool, 1 int, 2 float, 3 string */
     uint8_t flags;
 } obm_arg;
-enum { OBM_R_OK = 1, OBM_R_NL = 2, OBM_R_ERR_PARSEBOOL = 4, OBM_R_ERR_FLOAT32 = 8, OBM_R_HOST = 16 };
-enum { OBM_A_SYNTHETIC_TRUE = 1 };
+/* Typed definitions only (obm_registry_define):
+ *   OBM_R_ERR_SETARG   SetArgument failed: wrong type or FieldType unmarshal error (the formatter derives which from the
+ *                      argument's type and the value); ends the document's parse like the strconv errors
+ *   OBM_R_ERR_MISSING  InflateObject: required arguments never set (mask in aux); position {line:0 column:0}, MarkerText
+ *                      ends in the synthetic "\n" (OBM_R_NL); ends the document's parse
+ *   OBM_R_PANIC        SetArgument would panic in reflect.Set (an int for a string argument).  Not a Result in the
+ *                      reference: its process aborts.  Treat it as fatal for the whole run.
+ *   OBM_A_SUPERSEDED   an argument a later one of the same name overwrote (marker.go:59): the arguments of an OK result
+ *                      without it are exactly the fields InflateObject sets */
+enum { OBM_R_OK = 1, OBM_R_NL = 2, OBM_R_ERR_PARSEBOOL = 4, OBM_R_ERR_FLOAT32 = 8, OBM_R_HOST = 16, OBM_R_ERR_SETARG = 32,
+       OBM_R_ERR_MISSING = 64, OBM_R_PANIC = 128 };
+enum { OBM_A_SYNTHETIC_TRUE = 1, OBM_A_SUPERSEDED = 2 };
 /*
  * Per-document 64-bit hash of the DECODED lexeme stream, computed on the device from the resident tuples: FNV-1a over
  * the records [u8 type][u32 line][u32 col][u32 vlen][value] that obm_decode_doc serialises (and that the reference

@@ -14,7 +14,7 @@ EXPORTS = [
     "obm_scratch_bytes", "obm_generate_corpus_device", "obm_generate_corpus_host", "obm_set_mode", "obm_pinned_alloc", "obm_launches_last_call", "obm_set_chunk_bytes",
     "obm_pinned_free", "obm_stream_new", "obm_stream_next", "obm_stream_free", "obm_decode_doc", "obm_free", "obm_registry_new", "obm_registry_operator_builder", "obm_registry_add",
     "obm_comm_unique_id", "obm_comm_create", "obm_comm_destroy", "obm_lex_batch_sharded_device",
-    "obm_registry_free", "obm_parse_doc", "obm_hash_batch_device", "obm_parse_batch_device", "obm_results_format_doc", "obm_marker_index_device",
+    "obm_registry_free", "obm_registry_define", "obm_parse_doc", "obm_hash_batch_device", "obm_parse_batch_device", "obm_results_format_doc", "obm_marker_index_device",
     "obm_marker_index_flat_device", "obm_rewrite_collection_markers_device", "obm_split_docs_device", "obm_lex_collection_batch_device",
 ]
 
@@ -79,6 +79,7 @@ def lib():
     L.obm_registry_operator_builder.restype = vp
     L.obm_registry_add.argtypes = [vp, ctypes.c_char_p, ctypes.POINTER(ctypes.c_char_p), u32]
     L.obm_registry_free.argtypes = [vp]
+    L.obm_registry_define.argtypes = [vp, ctypes.c_int]
     L.obm_parse_doc.argtypes = [vp, vp, u64, vp, u64, ctypes.POINTER(ctypes.POINTER(ctypes.c_uint8)), ctypes.POINTER(u64)]
     L.obm_parse_doc.restype = ctypes.c_int64
     L.obm_rewrite_collection_markers_device.argtypes = [vp, vp, vp, u32, vp, u64, vp, vp]

@@ -26,6 +26,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <new>
+#include <type_traits>
 
 #include "../../include/obmarkers.h"
 #include "go_unicode_tables.h"
@@ -1666,15 +1667,18 @@ static int two_pass_scratch(obm_handle *h, uint32_t ndocs, cudaStream_t st, uint
 /* SURVEY.md 8(f) rank 1 proper: the parser on the device (csrc/obm_parse_dev.h), a thread per document */
 /* ------------------------------------------------------------------------------------------- */
 #include "obm_parse_dev.h"
-extern "C" bool obm_registry_flatten(const obm_registry *r, obmr::DevRegistry *D);
+extern "C" bool obm_registry_flatten(const obm_registry *r, obmr::DevTypedRegistry *D);
 /* A thread per document, as many threads as the SM holds: the walk is a dependent chain of ~180 tuple reads per document,
  * i.e. latency-bound -- what hides the latency is the number of documents in flight, not staging (a version that staged 32
  * documents' tuples per warp in 48 KiB of shared memory ran at 4 warps per SM and was 11x slower). */
 constexpr uint32_t PD_WARPS = 2, PD_CAP = 6144; /* k_hash_docs: warps per block; tuples staged per warp (48 KiB) */
-template <bool WRITE>
+/* TYPED: the registry holds a definition added with its Go struct type (obm_registry_define); the untyped walk takes the
+ * registry without the type bytes, so its parameter block is the one it had before typing existed */
+template <bool TYPED> using ParseRegistry = std::conditional_t<TYPED, obmr::DevTypedRegistry, obmr::DevRegistry>;
+template <bool WRITE, bool TYPED>
 __global__ void __launch_bounds__(128)
 k_parse_docs(const uint8_t *__restrict__ bytes, const uint64_t *__restrict__ doc_off, uint32_t ndocs, uint32_t doc_base,
-             const obm_tuple *__restrict__ tuples, const uint64_t *__restrict__ tuple_off, const __grid_constant__ obmr::DevRegistry R,
+             const obm_tuple *__restrict__ tuples, const uint64_t *__restrict__ tuple_off, const __grid_constant__ ParseRegistry<TYPED> R,
              uint32_t *__restrict__ cnt_res, uint32_t *__restrict__ cnt_args, const uint64_t *__restrict__ res_off, const uint64_t *__restrict__ arg_off,
              obm_result *__restrict__ res, uint64_t res_cap, obm_arg *__restrict__ args, uint64_t arg_cap) {
     const uint32_t d = blockIdx.x * blockDim.x + threadIdx.x;
@@ -1685,7 +1689,11 @@ k_parse_docs(const uint8_t *__restrict__ bytes, const uint64_t *__restrict__ doc
         S.res = res; S.args = args; S.res_at = res_off[d]; S.arg_at = arg_off[d];
         S.res_end = res_off[d + 1] < res_cap ? res_off[d + 1] : res_cap; S.arg_end = arg_off[d + 1] < arg_cap ? arg_off[d + 1] : arg_cap;
     }
-    obmr::parse_doc(R, bytes + doc_off[d], tuples + t0, (uint32_t)(tuple_off[d + 1] - t0), d + doc_base, S);
+    if constexpr (TYPED) {
+        obmr::TypedSink TS; static_cast<obmr::Sink &>(TS) = S;
+        obmr::parse_doc<true>(R, bytes + doc_off[d], tuples + t0, (uint32_t)(tuple_off[d + 1] - t0), d + doc_base, TS);
+        S.nres = TS.nres; S.nargs = TS.nargs;
+    } else obmr::parse_doc<false>(R, bytes + doc_off[d], tuples + t0, (uint32_t)(tuple_off[d + 1] - t0), d + doc_base, S);
     if (!WRITE) { cnt_res[d] = S.nres; cnt_args[d] = S.nargs; }
 }
 
@@ -1763,7 +1771,7 @@ extern "C" int obm_parse_batch_device(obm_handle *h, const obm_registry *reg, co
                                       const void *d_tuples, const void *d_doc_tuple_off, void *d_results, uint64_t res_cap, void *d_args, uint64_t arg_cap,
                                       void *d_doc_res_off, void *d_totals, void *stream) {
     if (!h || !reg || !d_doc_off || !d_doc_tuple_off || !d_doc_res_off) return OBM_E_ARG;
-    obmr::DevRegistry R;
+    obmr::DevTypedRegistry R;
     if (!obm_registry_flatten(reg, &R)) { set_err(h, "registry too large for the device parser (8 markers, 64 arguments, 1024 bytes of names)"); return OBM_E_ARG; }
     OBM_CUDA(h, cudaSetDevice(h->device));
     cudaStream_t st = (cudaStream_t)stream;
@@ -1780,8 +1788,15 @@ extern "C" int obm_parse_batch_device(obm_handle *h, const obm_registry *reg, co
     uint64_t *aoff = (uint64_t *)q; q += align_up(((uint64_t)ndocs + 1) * 8, 256);
     uint64_t *tile_sums = (uint64_t *)q;
     const uint32_t nb = (ndocs + 127) / 128, nt = scan_tiles(ndocs);
-    k_parse_docs<false><<<nb, 128, 0, st>>>((const uint8_t *)d_bytes, (const uint64_t *)d_doc_off, ndocs, doc_base, (const obm_tuple *)d_tuples,
-                                            (const uint64_t *)d_doc_tuple_off, R, cres, carg, nullptr, nullptr, nullptr, 0, nullptr, 0);
+    bool typed = false;
+    for (uint32_t i = 0; i < R.n; i++) typed = typed || R.typed[i];
+    const obmr::DevRegistry &RN = R; /* the untyped walk's parameter: the registry without its type bytes */
+    if (typed)
+        k_parse_docs<false, true><<<nb, 128, 0, st>>>((const uint8_t *)d_bytes, (const uint64_t *)d_doc_off, ndocs, doc_base, (const obm_tuple *)d_tuples,
+                                                      (const uint64_t *)d_doc_tuple_off, R, cres, carg, nullptr, nullptr, nullptr, 0, nullptr, 0);
+    else
+        k_parse_docs<false, false><<<nb, 128, 0, st>>>((const uint8_t *)d_bytes, (const uint64_t *)d_doc_off, ndocs, doc_base, (const obm_tuple *)d_tuples,
+                                                       (const uint64_t *)d_doc_tuple_off, RN, cres, carg, nullptr, nullptr, nullptr, 0, nullptr, 0);
     k_scan_tiles<<<nt, SCAN_THREADS, 0, st>>>(cres, ndocs, roff, tile_sums);
     k_scan_sums<<<1, SCAN_THREADS, 0, st>>>(tile_sums, nt, roff + ndocs);
     k_scan_add<<<nt, SCAN_THREADS, 0, st>>>(roff, ndocs, tile_sums, ~0ull, nullptr);
@@ -1792,10 +1807,14 @@ extern "C" int obm_parse_batch_device(obm_handle *h, const obm_registry *reg, co
         OBM_CUDA(h, cudaMemcpyAsync(d_totals, roff + ndocs, 8, cudaMemcpyDeviceToDevice, st));
         OBM_CUDA(h, cudaMemcpyAsync((uint64_t *)d_totals + 1, aoff + ndocs, 8, cudaMemcpyDeviceToDevice, st));
     }
-    if (d_results && d_args)
-        k_parse_docs<true><<<nb, 128, 0, st>>>((const uint8_t *)d_bytes, (const uint64_t *)d_doc_off, ndocs, doc_base, (const obm_tuple *)d_tuples,
-                                               (const uint64_t *)d_doc_tuple_off, R, cres, carg, roff, aoff, (obm_result *)d_results, res_cap,
-                                               (obm_arg *)d_args, arg_cap);
+    if (d_results && d_args && typed)
+        k_parse_docs<true, true><<<nb, 128, 0, st>>>((const uint8_t *)d_bytes, (const uint64_t *)d_doc_off, ndocs, doc_base, (const obm_tuple *)d_tuples,
+                                                     (const uint64_t *)d_doc_tuple_off, R, cres, carg, roff, aoff, (obm_result *)d_results, res_cap,
+                                                     (obm_arg *)d_args, arg_cap);
+    else if (d_results && d_args)
+        k_parse_docs<true, false><<<nb, 128, 0, st>>>((const uint8_t *)d_bytes, (const uint64_t *)d_doc_off, ndocs, doc_base, (const obm_tuple *)d_tuples,
+                                                      (const uint64_t *)d_doc_tuple_off, RN, cres, carg, roff, aoff, (obm_result *)d_results, res_cap,
+                                                      (obm_arg *)d_args, arg_cap);
     OBM_CUDA(h, cudaGetLastError());
     return OBM_OK;
 }

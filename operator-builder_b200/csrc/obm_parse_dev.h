@@ -7,6 +7,10 @@
  *   value typing               state.go:95-153 (ParseBool, Atoi class, ParseFloat(., 32) range)
  *   MarkerText                 position.go:18 + emit.go:8-24, as a span of the document (+ the synthetic "\n")
  *   error results              error.go:8-22 (they end the document's parse, parser.go:63-73)
+ * and, for definitions added with their Go struct types (obm_registry_define; the parse_doc<true> instantiation):
+ *   SetArgument                marker.go:53-63 -> argument.go:91-127 (wrong type, FieldType unmarshal, the int -> string panic)
+ *   InflateObject              marker.go:65-95 (required arguments never set), run by emit.go:8-24
+ *   last writer wins           marker.go:59 (Fields[argName] = arg): earlier writers of a field get OBM_A_SUPERSEDED
  * The same source is the host mirror's fast path (obm_parse.cpp: obm_results_format_doc) and is checked against
  * obm_parse_doc / oracle/parser_oracle.py in tests/test_parser_row.py.
  *
@@ -25,6 +29,32 @@ namespace obmr {
 struct DevRegistry { /* names and argument names back to back in text[] */
     uint32_t n; uint32_t name_off[9]; uint32_t arg_first[9]; uint32_t arg_off[65]; uint8_t text[1024];
 };
+/* The Go type of each argument of a typed definition (obm_registry_define), appended after text[]: the untyped walk is
+ * given the DevRegistry part alone, so its kernel parameter is what it was before typing existed.
+ * type[a] = TY_* | TY_REQUIRED; 0 = an argument of an untyped definition (every SetArgument succeeds). */
+enum : uint8_t { TY_NONE = 0, TY_STRING = 1 /* string, *string */, TY_BOOL = 2 /* *bool */, TY_FIELDTYPE = 3 /* markers.FieldType */,
+                 TY_ANY = 4 /* interface{} */, TY_KIND = 7, TY_REQUIRED = 0x80 };
+constexpr uint32_t TY_MAX_FIELDS = 5; /* the largest typed definition (FieldMarker) */
+struct DevTypedRegistry : DevRegistry {
+    uint8_t type[64];
+    uint8_t required[8]; /* per definition: bit j = argument j is required (InflateObject's missingFields) */
+    uint8_t typed[8];    /* per definition: 1 = added with its Go struct type */
+};
+/* SetArgument outcome of a value of lexeme kind vk (0 bool, 1 int, 2 float, 3 string) for an argument of type ty
+ * (argument.go:91-127 with the Go spec's conversion / assignability rules): 0 ok, 1 error (OBM_R_ERR_SETARG), 2 panic */
+OBM_HD uint32_t setarg_outcome(uint32_t ty, uint32_t vk, const uint8_t *v, uint32_t n) {
+    switch (ty & TY_KIND) {
+    case TY_STRING: return vk == 3 ? 0u : vk == 1 ? 2u : 1u; /* int is ConvertibleTo string but not assignable: reflect.Set panics */
+    case TY_BOOL: return vk == 0 ? 0u : 1u;
+    case TY_FIELDTYPE: /* (*FieldType).UnmarshalMarkerArg, field_types.go:27-46: "string", "int", "bool" */
+        if (vk != 3) return 1u;
+        if (n == 6) return (v[0] == 's' && v[1] == 't' && v[2] == 'r' && v[3] == 'i' && v[4] == 'n' && v[5] == 'g') ? 0u : 1u;
+        if (n == 3) return (v[0] == 'i' && v[1] == 'n' && v[2] == 't') ? 0u : 1u;
+        if (n == 4) return (v[0] == 'b' && v[1] == 'o' && v[2] == 'o' && v[3] == 'l') ? 0u : 1u;
+        return 1u;
+    default: return 0u; /* interface{}, untyped definitions */
+    }
+}
 
 OBM_HD bool slice_eq(const uint8_t *doc, uint32_t off, uint32_t len, const uint8_t *t, uint32_t tlen) {
     if (len != tlen) return false;
@@ -103,6 +133,9 @@ struct Sink {
         }
         nargs++;
     }
+    OBM_HD void supersede(uint32_t slot) { /* slot: index among this document's arguments */
+        if (args && arg_at + slot < arg_end) args[arg_at + slot].flags |= (uint8_t)OBM_A_SUPERSEDED;
+    }
     OBM_HD void result(uint32_t doc, uint32_t tuple, uint32_t text_off, uint32_t text_len, uint32_t reg_id, uint32_t n_args, uint64_t arg_base, uint32_t flags, uint32_t aux) {
         if (res && res_at + nres < res_end) {
             obm_result r; r.doc = doc; r.tuple = tuple; r.text_off = text_off; r.text_len = text_len; r.reg_id = (uint16_t)reg_id; r.nargs = (uint16_t)n_args;
@@ -111,6 +144,16 @@ struct Sink {
         }
         nres++;
     }
+};
+
+/* the typed walk's sink also carries SetArgument / InflateObject's state of the marker being parsed (kept out of the untyped
+ * walk's frame, which stays as it was) */
+struct TypedSink : Sink {
+    uint32_t a_idx = 0;                 /* registry index of the argument being valued */
+    uint32_t set_mask = 0;              /* fields set so far (argument index in the definition) */
+    uint64_t last = 0;                  /* the last writers of fields 0-3, 16 bits each: the writer's index among the marker's
+                                           arguments (< 2^16 like obm_result.nargs); packed, so the walk keeps them in registers */
+    uint32_t last4 = 0;                 /* and of field 4 */
 };
 
 /* 8 bytes of the document at an arbitrary offset (two aligned loads + funnel shift; the batch buffer is readable up to the
@@ -135,8 +178,11 @@ OBM_HD bool slice_eq8(const uint8_t *doc, uint32_t off, uint32_t len, const uint
  * Written as a DFA that consumes exactly ONE tuple per iteration of the outer loop (a state may hand the same tuple to
  * another state first: the parser's "peeked, not consumed" moves): a warp runs 32 documents, one per lane, and with one
  * tuple per iteration the lanes stay converged on the loop -- the walk is latency-bound on the tuple loads, which now issue
- * for all lanes at once. */
-OBM_HD void parse_doc(const DevRegistry &R, const uint8_t *doc, const obm_tuple *t, uint32_t nt, uint32_t doc_id, Sink &S) {
+ * for all lanes at once.
+ * TYPED (Reg = DevTypedRegistry, SinkT = TypedSink) adds SetArgument / InflateObject; TYPED = false (DevRegistry, Sink)
+ * compiles to the walk that has no types. */
+template <bool TYPED, class Reg, class SinkT>
+OBM_HD void parse_doc(const Reg &R, const uint8_t *doc, const obm_tuple *t, uint32_t nt, uint32_t doc_id, SinkT &S) {
     enum St { P_PARSE, P_MSTART, P_SCOPE, P_SEP, P_ARG, P_AV1, P_AV2, P_VAL, P_VQ, P_MORE };
     uint32_t line = 1, base = 0;                                                  /* position basis (LINE tuples) */
     uint32_t sc_off = 0, sc_len = 0; bool sc_any = false, sc_nl = false, sc_broken = false; /* scopeBuffer as a span (+ "\n") */
@@ -170,7 +216,7 @@ OBM_HD void parse_doc(const DevRegistry &R, const uint8_t *doc, const obm_tuple 
                     def = -1;
                     for (uint32_t r = 0; r < R.n; r++)
                         if (slice_eq8(doc, sc_off, sc_len - 1, R.text + R.name_off[r], R.name_off[r + 1] - R.name_off[r])) { def = (int)r; break; }
-                    if (def >= 0) { n_args = 0; arg_base = S.arg_at + S.nargs; st = P_ARG; }
+                    if (def >= 0) { n_args = 0; arg_base = S.arg_at + S.nargs; st = P_ARG; if constexpr (TYPED) S.set_mask = 0; }
                 }
                 if (st == P_PARSE) { sc_any = false; sc_nl = false; sc_len = 0; sc_broken = false; def = -1; } /* flush() */
                 break;
@@ -179,11 +225,36 @@ OBM_HD void parse_doc(const DevRegistry &R, const uint8_t *doc, const obm_tuple 
                 consumed = true; a_off = off; a_len = len;
                 st = P_PARSE;
                 for (uint32_t a = R.arg_first[def]; a < R.arg_first[def + 1]; a++)
-                    if (slice_eq8(doc, off, len, R.text + R.arg_off[a], R.arg_off[a + 1] - R.arg_off[a])) { st = P_AV1; break; }
+                    if (slice_eq8(doc, off, len, R.text + R.arg_off[a], R.arg_off[a + 1] - R.arg_off[a])) { st = P_AV1; if constexpr (TYPED) S.a_idx = a; break; }
                 break;
             case P_AV1: if (k == OBM_K_ARG_ASSIGNMENT) consumed = true; st = P_AV2; break;
             case P_AV2: if (k == OBM_K_QUOTE) consumed = true; st = P_VAL; break;
             case P_VAL: /* parseArgValue, state.go:95-153 */
+                if constexpr (TYPED) { /* SetArgument (marker.go:53-63, argument.go:91-127) on the value strconv produced */
+                    const uint32_t vk = k == OBM_K_SYNTHETIC_BOOL || k == OBM_K_BOOL_LITERAL ? 0u : k == OBM_K_INTEGER_LITERAL ? 1u
+                                      : k == OBM_K_FLOAT_LITERAL ? 2u : k == OBM_K_STRING_LITERAL ? 3u : 4u;
+                    const bool strconv_err = k == OBM_K_BOOL_LITERAL ? !parse_bool_ok(doc + off, len) : k == OBM_K_FLOAT_LITERAL && float32_overflows(doc + off, len);
+                    const uint32_t out = vk < 4 && !strconv_err ? setarg_outcome(R.type[S.a_idx], vk, doc + off, len) : 0u;
+                    if (out) { /* p.error: parser.current is the literal, or for the peeked synthetic bool the lexeme before it */
+                        const bool syn = k == OBM_K_SYNTHETIC_BOOL;
+                        if (!syn && len) { if (sc_any && !sc_nl && off == sc_off + sc_len) sc_len += len; else sc_broken = true; }
+                        if (sc_broken) { S.nres = 0; S.nargs = 0; S.result(doc_id, i, 0, 0, 0xFFFFu, 0, 0, OBM_R_HOST, 0); return; }
+                        S.nargs -= n_args;
+                        const uint64_t ab = S.arg_at + S.nargs;
+                        S.arg(syn ? cur_line : line, S.a_idx - R.arg_first[def], vk, off, syn ? 0u : len, syn ? (uint32_t)OBM_A_SYNTHETIC_TRUE : 0u);
+                        S.result(doc_id, syn ? cur_tuple : i, sc_off, sc_len, (uint32_t)def, 1, ab, out == 2 ? OBM_R_PANIC : OBM_R_ERR_SETARG,
+                                 syn ? cur_col : off - base + 1);
+                        return;
+                    }
+                    if (vk < 4 && !strconv_err && R.typed[def]) { /* Fields[argName] = arg (marker.go:59): the last writer wins */
+                        const uint32_t j = S.a_idx - R.arg_first[def];
+                        const uint32_t sh = 16u * (j & 3u);
+                        const uint32_t prev = j < 4 ? (uint32_t)(S.last >> sh) & 0xFFFFu : S.last4;
+                        if ((S.set_mask >> j) & 1u) S.supersede((uint32_t)(arg_base - S.arg_at) + prev);
+                        if (j < 4) S.last = (S.last & ~(0xFFFFull << sh)) | ((uint64_t)(n_args & 0xFFFFu) << sh); else S.last4 = n_args;
+                        S.set_mask |= 1u << j;
+                    }
+                }
                 if (k == OBM_K_SYNTHETIC_BOOL) { consumed = true; append = false; S.arg(a_off, a_len, 0, off, 0, OBM_A_SYNTHETIC_TRUE); n_args++; st = P_MORE; }
                 else if (k == OBM_K_BOOL_LITERAL || k == OBM_K_FLOAT_LITERAL) {
                     consumed = true;
@@ -227,6 +298,10 @@ OBM_HD void parse_doc(const DevRegistry &R, const uint8_t *doc, const obm_tuple 
                 if (was == P_PARSE && st == P_PARSE && k != OBM_K_COMMENT) { sc_any = false; sc_nl = false; sc_len = 0; sc_broken = false; } /* the catch-all of parse */
                 if (was == P_MORE && k == OBM_K_MARKER_END) { /* emit.go:8-24 */
                     if (sc_broken) { S.nres = 0; S.nargs = 0; S.result(doc_id, i, 0, 0, 0xFFFFu, 0, 0, OBM_R_HOST, 0); return; }
+                    if constexpr (TYPED) { /* InflateObject (marker.go:65-95): parser.current is the synthetic MarkerEnd, {line:0 column:0} */
+                        const uint32_t miss = R.required[def] & ~S.set_mask;
+                        if (miss) { S.nargs -= n_args; S.result(doc_id, i, sc_off, sc_len, (uint32_t)def, 0, S.arg_at + S.nargs, OBM_R_ERR_MISSING | OBM_R_NL, miss); return; }
+                    }
                     S.result(doc_id, marker_tuple, sc_off, sc_len, (uint32_t)def, n_args, arg_base, OBM_R_OK | OBM_R_NL, 0);
                     sc_any = false; sc_nl = false; sc_len = 0; sc_broken = false; def = -1; n_args = 0;
                 }

@@ -266,8 +266,31 @@ def generate_corpus_host(ndocs: int, doc_bytes: int = 4096, first_doc: int = 0, 
 
 
 # ---- the lexer's consumer: internal/markers/parser over the same tuple stream (SURVEY.md 8(f) rank 1) ----
+FIELD_MARKER, COLLECTION_MARKER, RESOURCE_MARKER = 0, 1, 2  # internal/workload/v1/markers/markers.go:20-25
+
+
 class Registry:
-    """marker.Registry stand-in (marker/registry.go:8-42): marker names (with '+') -> accepted argument names."""
+    """marker.Registry stand-in (marker/registry.go:8-42): marker names (with '+') -> accepted argument names.
+
+    Registry() and Registry({name: args}) hold names only: every argument value is accepted and every marker emits.
+    Registry.define(FIELD_MARKER, ...) holds the typed definitions marker.Define builds from operator-builder's structs,
+    so Results carry SetArgument / InflateObject's errors (include/obmarkers.h: obm_registry_define)."""
+
+    @classmethod
+    def define(cls, *marker_types):
+        """A registry of the typed definitions of `marker_types` (FIELD_MARKER, COLLECTION_MARKER, RESOURCE_MARKER), like
+        InspectForYAML(..., markerTypes...) builds (markers.go:92-113)."""
+        r = cls({})
+        for t in marker_types:
+            r.define_marker(t)
+        return r
+
+    def define_marker(self, marker_type: int):
+        """Add (or replace, by name) the typed definition of one marker type."""
+        rc = self._L.obm_registry_define(self._r, int(marker_type))
+        if rc != 0:
+            raise NativeError(rc, f"obm_registry_define: unknown marker type {marker_type}")
+        return self
 
     def __init__(self, markers=None):
         self._L = _native.lib()
