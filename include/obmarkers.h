@@ -194,19 +194,17 @@ void obm_pinned_free(void *p);
 int obm_rewrite_collection_markers_device(obm_handle *h, const void *d_bytes, const void *d_doc_off, uint32_t ndocs,
                                           void *d_out_bytes, uint64_t out_cap, void *d_out_doc_off, void *stream);
 /*
- * The collection rewrite above fused into the scan, for device-resident collection batches: one asynchronous call
- * whose outputs equal, bit for bit, what these two calls leave behind
+ * The collection rewrite above and the scan of its result, for device-resident collection batches: one call that is
+ * defined as these two calls, in every mode (obm_set_mode applies to the scan)
  *     obm_rewrite_collection_markers_device(h, d_bytes, d_doc_off, ndocs, d_out_bytes, out_bytes_cap, d_out_doc_off, stream)
  *     obm_lex_batch_device(h, d_out_bytes, d_out_doc_off, ndocs, <rewritten total>, d_out, out_cap, d_doc_tuple_off,
  *                          d_status, d_counts, stream)
  * i.e. the rewritten bytes and d_out_doc_off[ndocs+1], the tuple stream of the REWRITTEN documents (offsets relative to
- * them), d_doc_tuple_off, status and counts with obm_lex_batch_device's semantics.  One exception: status[1] (documents
- * the exact lexer took) also counts a document above the units' size limit whose rewritten text is below it (it stays
- * on the large path, which is exact at any size).  The text is read from memory once.
+ * them), d_doc_tuple_off, status and counts with obm_lex_batch_device's semantics.
  * d_bytes: as for obm_lex_batch_device.  d_out_bytes: 16-byte aligned, not overlapping d_bytes, out_bytes_cap >=
- * total_bytes (the rewrite never lengthens the text, so the bytes cannot overflow and the call does not synchronise);
- * OBM_E_ARG otherwise.  Nothing is written at or past d_out_doc_off[ndocs] in d_out_bytes.  Mode 0 returns after
- * enqueueing; modes 1-3 (obm_set_mode) run the two calls above.  Extra scratch is kept by the handle, grown on demand.
+ * total_bytes (the rewrite never lengthens the text, so the bytes cannot overflow); OBM_E_ARG otherwise.  Nothing is
+ * written at or past d_out_doc_off[ndocs] in d_out_bytes.  Synchronises the stream: the rewritten total, which sizes
+ * the scan, is read back between the two calls.
  */
 int obm_lex_collection_batch_device(obm_handle *h, const void *d_bytes, const void *d_doc_off, uint32_t ndocs, uint64_t total_bytes,
                                     void *d_out_bytes, uint64_t out_bytes_cap, void *d_out_doc_off,

@@ -374,7 +374,6 @@ struct obm_handle {
     char err[512];
     /* scratch kept across calls */
     void *scratch; uint64_t scratch_bytes;
-    void *rw_scratch; uint64_t rw_scratch_bytes; /* obm_lex_collection_batch_device: byte chain, large documents' rewritten text */
     /* device staging for the host-buffer entry point */
     uint8_t *d_bytes; uint64_t d_bytes_cap;
     uint64_t *d_doc_off; uint64_t d_doc_off_cap; /* elements */
@@ -454,7 +453,7 @@ extern "C" void obm_destroy(obm_handle *h) {
     if (!h) return;
     cudaSetDevice(h->device);
     cudaStreamSynchronize(h->stream);
-    cudaFree(h->scratch); cudaFree(h->rw_scratch); cudaFree(h->d_bytes); cudaFree(h->d_doc_off); cudaFree(h->d_tuple_off); cudaFree(h->d_out);
+    cudaFree(h->scratch); cudaFree(h->d_bytes); cudaFree(h->d_doc_off); cudaFree(h->d_tuple_off); cudaFree(h->d_out);
     cudaFree(h->d_status); cudaFree(h->d_counts);
     if (h->slots_ready) for (auto &sl : h->slots) {
         cudaStreamSynchronize(sl.st);
@@ -662,28 +661,14 @@ static uint64_t warp_scratch_bytes(uint32_t ndocs, uint64_t total_bytes) {
            align_up(((uint64_t)scan_tiles((uint32_t)nt) + 1) * 8, 256) + align_up((nt + 1) * sizeof(obmw::WRec), 256) + align_up((um + 1) * 8, 256) +
            align_up(2 * (um / 32 + 2) * 8, 256) + align_up((um + 1) * 4, 256) + 512;
 }
-/* the collection variant's outputs and its own scratch (obm_lex_collection_batch_device) */
-struct RwOut { uint8_t *out_bytes; uint64_t *out_doc_off; void *ws; };
-/* rw scratch: lg_len u32[ndocs] | lg_off u64[ndocs+1] | scan sums | byte chain (units, blocks) | large documents' rewritten text */
-static uint64_t rw_scratch_bytes(uint32_t ndocs, uint64_t total_bytes) {
-    const uint64_t um = warp_units_max(ndocs, total_bytes);
-    return align_up((uint64_t)ndocs * 4 + 4, 256) + align_up(((uint64_t)ndocs + 1) * 8, 256) + align_up(((uint64_t)scan_tiles(ndocs) + 1) * 8, 256) +
-           align_up((um + 1) * 8, 256) + align_up(2 * (um / 32 + 2) * 8, 256) + align_up(total_bytes + 64, 256);
-}
-static void large_rewrite_launch(cudaStream_t st, int sms, const uint8_t *d_bytes, const uint64_t *d_doc_off, uint32_t ndocs, const uint32_t *large_list,
-                                 const uint32_t *n_large, uint32_t max_large, uint32_t *lg_len, uint64_t *lg_off, uint64_t *lg_sums, uint8_t *lg_text);
-static void large_place_launch(cudaStream_t st, int sms, const uint8_t *lg_text, const uint64_t *lg_off, const uint32_t *large_list, const uint32_t *n_large,
-                               uint32_t max_large, uint8_t *out_bytes, const uint64_t *out_doc_off);
 /* tile index -> (large documents planned and counted on a side stream) units per tile + scan -> k_warp_scan -> fill of
- * the large documents.  REWRITE: the large documents are rewritten into rw scratch first (side stream) and lexed there;
- * k_warp_scan<true> rewrites the units; after it, the large documents' text is copied to its place. */
-template <bool REWRITE>
+ * the large documents */
 static int obm_warp_launch(obm_handle *h, const uint8_t *d_bytes, const uint64_t *d_doc_off, uint32_t ndocs, uint64_t total_bytes,
                            obm_tuple *d_out, uint64_t out_cap, uint64_t *toff, uint32_t *status, unsigned long long *totals,
-                           uint32_t *counts, void *warp_ws, void *large_ws, cudaStream_t st, const RwOut *rw) {
+                           uint32_t *counts, void *warp_ws, void *large_ws, cudaStream_t st) {
     static_assert(sizeof(obmw::WarpSmem) * obmw::WPC <= 232448, "the warps of the CTA share the 227 KB of one SM");
     const size_t smem = sizeof(obmw::WarpSmem) * obmw::WPC;
-    OBM_CUDA(h, cudaFuncSetAttribute(obmw::k_warp_scan<REWRITE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); /* per device: set on every call (cheap) */
+    OBM_CUDA(h, cudaFuncSetAttribute(obmw::k_warp_scan, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); /* per device: set on every call (cheap) */
     const uint64_t nt64 = warp_ntiles(total_bytes), um = warp_units_max(ndocs, total_bytes);
     if (nt64 > 0xFFFFFFF0ull || um > 0xFFFFFFF0ull) { set_err(h, "batch too large for the tile index"); return OBM_E_ARG; }
     const uint32_t ntiles = (uint32_t)nt64, nt_u = scan_tiles(ntiles);
@@ -704,55 +689,29 @@ static int obm_warp_launch(obm_handle *h, const uint8_t *d_bytes, const uint64_t
     A.st_blocks = (uint64_t *)q; q += up(2 * (um / 32 + 2) * 8); A.units_max = um;
     A.ctl = (uint32_t *)q; /* [0] ticket, [1] n_large */
     A.counts = counts; A.out = d_out; A.out_cap = d_out ? out_cap : 0; A.tuple_off = toff; A.status = status; A.totals = totals;
-    A.st_bytes = nullptr; A.st_bblocks = nullptr; A.lg_off = nullptr; A.out_bytes = nullptr; A.out_doc_off = nullptr;
     OBM_CUDA(h, cudaMemsetAsync(A.st_tuples, 0, up((um + 1) * 8) + up(2 * (um / 32 + 2) * 8) + 64, st)); /* chain arrays + control words */
-    const uint32_t max_large = (uint32_t)obm_fast_max_large(total_bytes);
-    uint32_t *lg_len = nullptr; uint64_t *lg_sums = nullptr; uint8_t *lg_text = nullptr;
-    if constexpr (REWRITE) {
-        uint8_t *r = (uint8_t *)rw->ws;
-        lg_len = (uint32_t *)r; r += up((uint64_t)ndocs * 4 + 4);
-        A.lg_off = (const uint64_t *)r; r += up(((uint64_t)ndocs + 1) * 8);
-        lg_sums = (uint64_t *)r; r += up(((uint64_t)scan_tiles(ndocs) + 1) * 8);
-        A.st_bytes = (uint64_t *)r; r += up((um + 1) * 8);
-        A.st_bblocks = (uint64_t *)r; r += up(2 * (um / 32 + 2) * 8);
-        lg_text = r;
-        A.out_bytes = rw->out_bytes; A.out_doc_off = rw->out_doc_off;
-        OBM_CUDA(h, cudaMemsetAsync(A.st_bytes, 0, up((um + 1) * 8) + up(2 * (um / 32 + 2) * 8), st)); /* the byte chain */
-    }
     obmw::k_wtile_index<<<(ndocs + 1 + 255) / 256, 256, 0, st>>>(d_doc_off, ndocs, ntiles, tile_first, large_list, A.ctl + 1);
     int dev_sms = 0, per_sm = 0;
     OBM_CUDA(h, cudaDeviceGetAttribute(&dev_sms, cudaDevAttrMultiProcessorCount, h->device));
     const LargeWs LW = large_carve(large_ws, total_bytes, large_list, A.ctl + 1);
     OBM_CUDA(h, cudaEventRecord(h->ev_fork, st));
     OBM_CUDA(h, cudaStreamWaitEvent(h->side, h->ev_fork, 0));
-    /* the large path reads the large documents through (lbytes, loff): for REWRITE their rewritten text at lg_off[d], which
-     * keeps the global document indices (lg_off is the exclusive prefix of "rewritten length if large, else 0") */
-    const uint8_t *lbytes = d_bytes; const uint64_t *loff = d_doc_off;
-    if constexpr (REWRITE) {
-        OBM_CUDA(h, cudaMemsetAsync(lg_len, 0, (uint64_t)ndocs * 4 + 4, h->side));
-        large_rewrite_launch(h->side, dev_sms, d_bytes, d_doc_off, ndocs, large_list, A.ctl + 1, max_large, lg_len, (uint64_t *)A.lg_off, lg_sums, lg_text);
-        lbytes = lg_text; loff = A.lg_off;
-    }
-    large_count_launch(h->side, dev_sms, lbytes, loff, LW, counts, totals, status);
+    large_count_launch(h->side, dev_sms, d_bytes, d_doc_off, LW, counts, totals, status);
     OBM_CUDA(h, cudaEventRecord(h->ev_join, h->side));
     obmw::k_wunits<<<(ntiles + 255) / 256, 256, 0, st>>>(d_doc_off, tile_first, ntiles, nun, wrec);
     k_scan_tiles<<<nt_u, SCAN_THREADS, 0, st>>>(nun, ntiles, ubase, usums);
     k_scan_sums<<<1, SCAN_THREADS, 0, st>>>(usums, nt_u, ubase + ntiles);
     k_scan_add<<<nt_u, SCAN_THREADS, 0, st>>>(ubase, ntiles, usums, ~0ull, nullptr);
     obmw::k_wunit_tiles<<<(ntiles + 255) / 256, 256, 0, st>>>(nun, ubase, ntiles, um, unit_tile);
-    OBM_CUDA(h, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, obmw::k_warp_scan<REWRITE>, (int)(obmw::WPC * 32), smem));
+    OBM_CUDA(h, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, obmw::k_warp_scan, (int)(obmw::WPC * 32), smem));
     if (per_sm < 1) per_sm = 1;
     uint32_t grid = (uint32_t)dev_sms * (uint32_t)per_sm; /* persistent warps: a multiple of the SM count */
     const uint32_t gmax = (uint32_t)((um < 0xFFFFFFF0ull ? um : 0xFFFFFFF0ull) + obmw::WPC - 1) / obmw::WPC;
     if (grid > gmax) grid = gmax;
     OBM_CUDA(h, cudaStreamWaitEvent(st, h->ev_join, 0));
-    obmw::k_warp_scan<REWRITE><<<grid, obmw::WPC * 32, smem, st>>>(A);
+    obmw::k_warp_scan<<<grid, obmw::WPC * 32, smem, st>>>(A);
     uint32_t launches = 7 + LARGE_COUNT_LAUNCHES;
-    if (d_out && out_cap) { large_fill_launch(st, dev_sms, lbytes, loff, LW, toff, d_out, out_cap); launches += 1; }
-    if constexpr (REWRITE) {
-        large_place_launch(st, dev_sms, lg_text, A.lg_off, large_list, A.ctl + 1, max_large, rw->out_bytes, rw->out_doc_off);
-        launches += 7;
-    }
+    if (d_out && out_cap) { large_fill_launch(st, dev_sms, d_bytes, d_doc_off, LW, toff, d_out, out_cap); launches += 1; }
     h->launches = launches;
     OBM_CUDA(h, cudaGetLastError());
     return OBM_OK;
@@ -770,8 +729,7 @@ extern "C" uint64_t obm_scratch_bytes(uint32_t ndocs, uint64_t total_bytes) {
 
 static int lex_device_impl(obm_handle *h, const void *d_bytes, const void *d_doc_off, uint32_t ndocs,
                            uint64_t total_bytes, void *d_out, uint64_t out_cap, void *d_doc_tuple_off,
-                           void *d_status, void *d_counts, cudaStream_t st, void **scratch_p = nullptr, uint64_t *scratch_bytes_p = nullptr,
-                           const RwOut *rw = nullptr) {
+                           void *d_status, void *d_counts, cudaStream_t st, void **scratch_p = nullptr, uint64_t *scratch_bytes_p = nullptr) {
     if (!h) return OBM_E_ARG;
     if (!d_doc_off || !d_doc_tuple_off || (ndocs && total_bytes && !d_bytes)) { set_err(h, "null device pointer"); return OBM_E_ARG; }
     OBM_CUDA(h, cudaSetDevice(h->device));
@@ -794,18 +752,11 @@ static int lex_device_impl(obm_handle *h, const void *d_bytes, const void *d_doc
     uint64_t *toff = (uint64_t *)d_doc_tuple_off;
     OBM_CUDA(h, cudaMemsetAsync(status, 0, 4 * sizeof(uint32_t), st));
     OBM_CUDA(h, cudaMemsetAsync(totals, 0, 2 * sizeof(unsigned long long), st));
-    if (ndocs == 0) {
-        OBM_CUDA(h, cudaMemsetAsync(toff, 0, sizeof(uint64_t), st));
-        if (rw) OBM_CUDA(h, cudaMemsetAsync(rw->out_doc_off, 0, sizeof(uint64_t), st));
-        return OBM_OK;
-    }
+    if (ndocs == 0) { OBM_CUDA(h, cudaMemsetAsync(toff, 0, sizeof(uint64_t), st)); return OBM_OK; }
 
-    if (rw) /* only in mode 0 (obm_lex_collection_batch_device) */
-        return obm_warp_launch<true>(h, (const uint8_t *)d_bytes, (const uint64_t *)d_doc_off, ndocs, total_bytes, (obm_tuple *)d_out, out_cap, toff, status,
-                                     totals, counts, warp_ws, large_ws, st, rw);
     if (h->mode == 0)
-        return obm_warp_launch<false>(h, (const uint8_t *)d_bytes, (const uint64_t *)d_doc_off, ndocs, total_bytes, (obm_tuple *)d_out, out_cap, toff, status,
-                                      totals, counts, warp_ws, large_ws, st, nullptr);
+        return obm_warp_launch(h, (const uint8_t *)d_bytes, (const uint64_t *)d_doc_off, ndocs, total_bytes, (obm_tuple *)d_out, out_cap, toff, status,
+                               totals, counts, warp_ws, large_ws, st);
     if (h->mode == 3)
         return obm_pipe_launch(h, (const uint8_t *)d_bytes, (const uint64_t *)d_doc_off, ndocs, total_bytes,
                                 (obm_tuple *)d_out, out_cap, toff, status, totals, counts, fast_ws, pipe_ws, large_ws, st);
@@ -1530,51 +1481,6 @@ k_rewrite_collection(const uint8_t *__restrict__ bytes, const uint64_t *__restri
         if (!WRITE && lane == 0) new_len[d] = o;
     }
 }
-/* the large documents of a collection batch (obm_lex_collection_batch_device), a warp each: rewritten lengths, then the
- * rewritten text into scratch at lg_off[d] */
-template <bool WRITE>
-__global__ void __launch_bounds__(256)
-k_rewrite_large(const uint8_t *__restrict__ bytes, const uint64_t *__restrict__ doc_off, const uint32_t *__restrict__ large_list,
-                const uint32_t *__restrict__ n_large, uint32_t *__restrict__ lg_len, const uint64_t *__restrict__ lg_off, uint8_t *__restrict__ lg_text) {
-    const uint32_t lane = threadIdx.x & 31;
-    const uint32_t warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, nwarps = (gridDim.x * blockDim.x) >> 5;
-    const uint32_t nl = *n_large;
-    for (uint32_t i = warp; i < nl; i += nwarps) {
-        const uint32_t d = large_list[i];
-        const uint32_t o = rewrite_doc_warp<WRITE>(bytes + doc_off[d], (uint32_t)(doc_off[d + 1] - doc_off[d]), WRITE ? lg_text + lg_off[d] : nullptr, lane);
-        if (!WRITE && lane == 0) lg_len[d] = o;
-    }
-}
-/* ... and after the scan, their rewritten text at its final place */
-__global__ void __launch_bounds__(256)
-k_place_large(const uint8_t *__restrict__ lg_text, const uint64_t *__restrict__ lg_off, const uint32_t *__restrict__ large_list,
-              const uint32_t *__restrict__ n_large, uint8_t *__restrict__ out_bytes, const uint64_t *__restrict__ out_doc_off) {
-    const uint32_t lane = threadIdx.x & 31;
-    const uint32_t warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, nwarps = (gridDim.x * blockDim.x) >> 5;
-    const uint32_t nl = *n_large;
-    for (uint32_t i = warp; i < nl; i += nwarps) {
-        const uint32_t d = large_list[i];
-        warp_copy_bytes(out_bytes + out_doc_off[d], lg_text + lg_off[d], (uint32_t)(lg_off[d + 1] - lg_off[d]), lane);
-    }
-}
-static uint32_t large_warps_grid(int sms, uint32_t max_large) {
-    uint32_t nb = (uint32_t)sms * 8u, need = (max_large + 7) / 8;
-    if (nb > need) nb = need;
-    return nb ? nb : 1u;
-}
-static void large_rewrite_launch(cudaStream_t st, int sms, const uint8_t *d_bytes, const uint64_t *d_doc_off, uint32_t ndocs, const uint32_t *large_list,
-                                 const uint32_t *n_large, uint32_t max_large, uint32_t *lg_len, uint64_t *lg_off, uint64_t *lg_sums, uint8_t *lg_text) {
-    const uint32_t nb = large_warps_grid(sms, max_large), nt = scan_tiles(ndocs);
-    k_rewrite_large<false><<<nb, 256, 0, st>>>(d_bytes, d_doc_off, large_list, n_large, lg_len, nullptr, nullptr);
-    k_scan_tiles<<<nt, SCAN_THREADS, 0, st>>>(lg_len, ndocs, lg_off, lg_sums);
-    k_scan_sums<<<1, SCAN_THREADS, 0, st>>>(lg_sums, nt, lg_off + ndocs);
-    k_scan_add<<<nt, SCAN_THREADS, 0, st>>>(lg_off, ndocs, lg_sums, ~0ull, nullptr);
-    k_rewrite_large<true><<<nb, 256, 0, st>>>(d_bytes, d_doc_off, large_list, n_large, nullptr, lg_off, lg_text);
-}
-static void large_place_launch(cudaStream_t st, int sms, const uint8_t *lg_text, const uint64_t *lg_off, const uint32_t *large_list, const uint32_t *n_large,
-                               uint32_t max_large, uint8_t *out_bytes, const uint64_t *out_doc_off) {
-    k_place_large<<<large_warps_grid(sms, max_large), 256, 0, st>>>(lg_text, lg_off, large_list, n_large, out_bytes, out_doc_off);
-}
 
 /* Each record: { u32 doc, u32 a, u32 b, u32 0 }: extracted manifest = "\n" + content[a:b) (ExtractManifests
  * rebuilds it as "\n" + line for every line between separators; a separator is a line that equals "---" after
@@ -1886,9 +1792,9 @@ extern "C" int obm_rewrite_collection_markers_device(obm_handle *h, const void *
     return OBM_OK;
 }
 
-/* Manifest.LoadContent's collection rewrite fused into the scan: the same outputs as obm_rewrite_collection_markers_device
- * followed by obm_lex_batch_device over its result, with the text read from memory once.  Mode 0: k_warp_scan<true>,
- * asynchronous; modes 1-3 (a test switch): that composition itself. */
+/* Manifest.LoadContent's collection rewrite and the scan of its result: obm_rewrite_collection_markers_device, then
+ * obm_lex_batch_device over the rewritten batch (in the handle's mode).  Synchronous: the scan is sized by the
+ * rewritten total, read back from the device. */
 extern "C" int obm_lex_collection_batch_device(obm_handle *h, const void *d_bytes, const void *d_doc_off, uint32_t ndocs, uint64_t total_bytes,
                                                void *d_out_bytes, uint64_t out_bytes_cap, void *d_out_doc_off, void *d_out, uint64_t out_cap,
                                                void *d_doc_tuple_off, void *d_status, void *d_counts, void *stream) {
@@ -1902,24 +1808,14 @@ extern "C" int obm_lex_collection_batch_device(obm_handle *h, const void *d_byte
     const uintptr_t in0 = (uintptr_t)d_bytes, out0 = (uintptr_t)d_out_bytes;
     if (total_bytes && in0 < out0 + out_bytes_cap && out0 < in0 + total_bytes) { set_err(h, "d_out_bytes overlaps d_bytes"); return OBM_E_ARG; }
     cudaStream_t st = (cudaStream_t)stream;
-    if (h->mode != 0) {
-        int rc = obm_rewrite_collection_markers_device(h, d_bytes, d_doc_off, ndocs, d_out_bytes, out_bytes_cap, d_out_doc_off, stream);
-        if (rc != OBM_OK) return rc;
-        uint64_t rewritten = 0;
-        if (ndocs) {
-            OBM_CUDA(h, cudaMemcpyAsync(&rewritten, (const uint64_t *)d_out_doc_off + ndocs, 8, cudaMemcpyDeviceToHost, st));
-            OBM_CUDA(h, cudaStreamSynchronize(st));
-        }
-        return obm_lex_batch_device(h, d_out_bytes, d_out_doc_off, ndocs, rewritten, d_out, out_cap, d_doc_tuple_off, d_status, d_counts, stream);
+    int rc = obm_rewrite_collection_markers_device(h, d_bytes, d_doc_off, ndocs, d_out_bytes, out_bytes_cap, d_out_doc_off, stream);
+    if (rc != OBM_OK) return rc;
+    uint64_t rewritten = 0;
+    if (ndocs) {
+        OBM_CUDA(h, cudaMemcpyAsync(&rewritten, (const uint64_t *)d_out_doc_off + ndocs, 8, cudaMemcpyDeviceToHost, st));
+        OBM_CUDA(h, cudaStreamSynchronize(st));
     }
-    OBM_CUDA(h, cudaSetDevice(h->device));
-    const uint64_t need = rw_scratch_bytes(ndocs, total_bytes);
-    if (h->rw_scratch_bytes < need) {
-        if (h->rw_scratch) { OBM_CUDA(h, cudaStreamSynchronize(st)); cudaFree(h->rw_scratch); h->rw_scratch = nullptr; h->rw_scratch_bytes = 0; }
-        OBM_CUDA(h, cudaMalloc(&h->rw_scratch, need)); h->rw_scratch_bytes = need;
-    }
-    const RwOut rw{(uint8_t *)d_out_bytes, (uint64_t *)d_out_doc_off, h->rw_scratch};
-    return lex_device_impl(h, d_bytes, d_doc_off, ndocs, total_bytes, d_out, out_cap, d_doc_tuple_off, d_status, d_counts, st, nullptr, nullptr, &rw);
+    return obm_lex_batch_device(h, d_out_bytes, d_out_doc_off, ndocs, rewritten, d_out, out_cap, d_doc_tuple_off, d_status, d_counts, stream);
 }
 
 extern "C" int obm_split_docs_device(obm_handle *h, const void *d_bytes, const void *d_doc_off, uint32_t ndocs, void *d_records, uint64_t cap,

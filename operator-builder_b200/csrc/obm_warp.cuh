@@ -6,11 +6,9 @@
  *   k_wunit_tiles   unit -> tile
  *   k_warp_scan     persistent warps (no block barrier anywhere): a warp takes a unit by ticket, stages the text of
  *                   each of its units with one TMA bulk copy (cp.async.bulk + mbarrier) into its own slice of shared
- *                   memory and runs obmw::process_unit on it; k_warp_scan<true> also applies the collection rewrite to
- *                   the staged text and writes the rewritten text out (obm_lex_collection_batch_device)
+ *                   memory and runs obmw::process_unit on it
  */
 #pragma once
-#include <type_traits>
 #include "obm_fast.cuh"
 #include "obm_pipe.cuh"
 
@@ -77,10 +75,6 @@ struct DevHooks {
         if (nbytes) { obmf::mbar_wait(&S.mbar, phase); phase ^= 1u; }
     }
 };
-struct DevHooksRw : DevHooks { /* compute_unit<true>: the rewritten byte count goes on the byte chain right after the compaction */
-    uint64_t *st_bytes, *st_bblocks;
-    __device__ __forceinline__ void publish_bytes(uint32_t u, uint64_t n);
-};
 
 /* ---- the chain over the units' tuple counts ---------------------------------------------------------------
  * Two levels, both fed at PUBLISH time so that nothing on it depends on another warp's (deferred) resolve:
@@ -88,8 +82,7 @@ struct DevHooksRw : DevHooks { /* compute_unit<true>: the rewritten byte count g
  *   blk[b]   atomic accumulator of block b = units [32b, 32b+32): count << 56 | sum of tuples
  *   bex[b]   BEX_FLAG | exclusive prefix of block b, stored by whichever unit of the block resolves it first
  * resolve(u) = bex[b] (or a walk back over complete blocks, 32 per step, down to the nearest stored prefix) + the
- * st0 entries of the earlier units of u's own block.
- * k_warp_scan<true> runs a second chain of the same shape over the units' rewritten byte counts (A.st_bytes, A.st_bblocks). */
+ * st0 entries of the earlier units of u's own block. */
 #define BEX_FLAG (1ull << 63)
 __device__ __forceinline__ void chain_publish(uint64_t *st_units, uint64_t *st_blocks, uint32_t u, uint64_t total) {
     if ((threadIdx.x & 31) == 0) {
@@ -143,12 +136,6 @@ __device__ __forceinline__ uint64_t chain_resolve(uint64_t *st_units, uint64_t *
  * write unit i-1 from W.fin (its exclusive prefix has had a whole unit's time to arrive: no waiting on the chain),
  * assemble unit i into W.fin, scan unit i+1 ...  A unit whose write needs the staged text (documents for the exact
  * lexer, marker lines that are not staged) or that does not fit W.fin is written at once instead. */
-__device__ __forceinline__ void DevHooksRw::publish_bytes(uint32_t u, uint64_t n) { chain_publish(st_bytes, st_bblocks, u, n); }
-
-/* REWRITE (the collection variant, obm_lex_collection_batch_device): compute_unit compacts the staged text before phase
- * A and publishes its byte count on the second chain; the rewritten text leaves shared memory (write_text) before the
- * next unit's bulk copy overwrites it.  k_warp_scan<false> is the plain scan. */
-template <bool REWRITE>
 __global__ void __launch_bounds__(WPC * 32, 1) /* one CTA per SM: ptxas may take the registers it wants (151 on sm_90a; without the hint it settles for fewer and spills) */
 k_warp_scan(WArgs A) {
     extern __shared__ __align__(16) uint8_t smem_raw[];
@@ -159,9 +146,7 @@ k_warp_scan(WArgs A) {
     const obm::Tables T = obmq::dev_tables();
     const uint32_t nunits = (uint32_t)A.ubase[A.ntiles];
     const uint32_t nblocks = (uint32_t)(A.units_max / 32 + 2); /* layout of st_blocks: blk[nblocks] | bex[nblocks] */
-    std::conditional_t<REWRITE, DevHooksRw, DevHooks> H;
-    H.phase = 0;
-    if constexpr (REWRITE) { H.st_bytes = A.st_bytes; H.st_bblocks = A.st_bblocks; }
+    DevHooks H{0};
     WAcc acc{0, 0, 0, 0};
     UnitRegs pend; bool have_pend = false;
     /* unit iterator: UNITS by ticket, in document order (not tiles: a warp that held two units of one tile would publish
@@ -191,9 +176,8 @@ k_warp_scan(WArgs A) {
         const UnitDesc nxt = next_unit();
         OBMW_PC_MARK(PC_OTHER);
         UnitRegs R;
-        compute_unit<REWRITE>(S, S.set, A, T, H, cur, prestaged, R OBMW_PC_ARG);
+        compute_unit(S, S.set, A, T, H, cur, prestaged, R OBMW_PC_ARG);
         chain_publish(A.st_tuples, A.st_blocks, R.u, R.total);
-        if constexpr (REWRITE) write_text(S, A, R, chain_resolve(A.st_bytes, A.st_bblocks, R.u, nblocks));
         prestaged = false;
         /* the staged text is dead unless this unit's write needs it: bring in the next unit's text under the assembly and the writes */
         if (!R.needs_text && nxt.valid && nxt.db > nxt.da) { H.stage(S, (const void *)(uintptr_t)nxt.base_abs, desc_load(nxt)); prestaged = true; }

@@ -42,7 +42,7 @@ namespace obmw {
 constexpr uint32_t TILE = OBMW_TILE;      /* a unit = the documents starting in [t*TILE, (t+1)*TILE) (split when > DMAX / > BUFB) */
 constexpr uint32_t BUFB = OBMW_BUFB;      /* bytes of text staged per warp */
 constexpr uint32_t MAXDOC = (BUFB - 16 < 16368u) ? BUFB - 16 : 16368u; /* larger documents take the chunk-parallel exact path */
-constexpr uint32_t ROW = 1024;            /* bytes per bitmap row: 32 words, one W.naw entry (rewrite_staged steps by rows, 32 bytes per lane) */
+constexpr uint32_t ROW = 1024;            /* bytes per bitmap row: 32 words, one W.naw entry */
 constexpr uint32_t STEP = 2048;           /* bytes per phase-A step: 64 per lane, words 2L and 2L+1 (one W.nlpre entry) */
 constexpr uint32_t NWORDS = BUFB / 32;    /* 32-byte words of the bitmaps */
 constexpr uint32_t DMAX = 31;             /* documents per unit: one lane each, lane nd holds the end */
@@ -109,13 +109,11 @@ struct DirectSink {
 #define OBMW_FFS64(x) ((uint32_t)__ffsll((long long)(x)))
 #define OBMW_POPC64(x) ((uint32_t)__popcll(x))
 #define OBMW_FUNNEL_L(lo, hi, s) __funnelshift_l((lo), (hi), (s))
-#define OBMW_FUNNEL_R(lo, hi, s) __funnelshift_r((lo), (hi), (s))
 #else
 #define OBMW_FFS(x) ((uint32_t)__builtin_ffs((int)(x)))
 #define OBMW_FFS64(x) ((uint32_t)__builtin_ffsll((long long)(x)))
 #define OBMW_POPC64(x) ((uint32_t)__builtin_popcountll(x))
 #define OBMW_FUNNEL_L(lo, hi, s) ((uint32_t)(((((uint64_t)(hi)) << 32) | (uint64_t)(lo)) << ((s) & 31) >> 32))
-#define OBMW_FUNNEL_R(lo, hi, s) ((uint32_t)(((((uint64_t)(hi)) << 32) | (uint64_t)(lo)) >> ((s) & 31)))
 #endif
 
 /* ---- A: byte classes of 32 bytes (8 little-endian words) ------------------------------------------------ */

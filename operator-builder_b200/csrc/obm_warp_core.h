@@ -12,12 +12,7 @@
  * and supplies a Hooks type with
  *     stage(W, gsrc, nbytes) bring nbytes (multiple of 16) from the 16-byte aligned global address gsrc into W.text
  *     stage_wait(W, nbytes)  ... and wait for them
- *     publish_bytes(u, n)    (compute_unit<true> only) unit u's rewritten byte count, as soon as it is known
  * The look-back chain over the units' tuple counts is driven by the caller between compute_unit and write_unit.
- *
- * compute_unit<true> is the collection variant: Manifest.LoadContent's rewrite (obm_rewrite.cuh) is applied to the
- * staged text before phase A (rewrite_staged), so every later phase sees the rewritten documents; write_text then
- * puts the rewritten text at its final place.
  */
 #ifndef OBM_WARP_CORE_H
 #define OBM_WARP_CORE_H
@@ -83,7 +78,6 @@ struct UnitRegs {
     uint32_t u, da, nd, extra, n_owners, n_ml, n_small /* tuples of the unit's small documents */; uint64_t total; bool needs_text;
     bool paged; /* more owning lines than OWN_CAP: the unit is scanned (and later written) one document at a time */
     uint32_t dflag, dtot, dexcl, dlen; /* lane d < nd: document da + d */
-    uint32_t kept; uint64_t nbytes;    /* REWRITE: rewritten bytes of the unit's small documents; ... and of its large one too */
 };
 
 struct WArgs {
@@ -96,10 +90,6 @@ struct WArgs {
     const uint32_t *counts;                  /* tuple counts of large documents (k_large_resolve) */
     obm_tuple *out; uint64_t out_cap; uint64_t *tuple_off;
     uint32_t *status; unsigned long long *totals; uint32_t *ctl;
-    /* REWRITE only (k_warp_scan<true>): the collection rewrite fused into the scan */
-    uint64_t *st_bytes, *st_bblocks;         /* second chain, over the units' rewritten byte counts */
-    const uint64_t *lg_off;                  /* [ndocs + 1] exclusive prefix of "rewritten length if large, else 0" */
-    uint8_t *out_bytes; uint64_t *out_doc_off; /* the rewritten batch (16-byte aligned) and its document offsets */
 };
 /* where a unit's text lies: computed ahead of the unit so that its bulk copy can be issued early */
 struct UnitDesc { uint32_t u, da, db, extra, skew, span; uint64_t base_abs; bool valid; };
@@ -467,100 +457,8 @@ OBMW_DEV bool scan_range(WarpSmem &W, UnitSet &S, const WArgs &A, const obm::Tab
     return true;
 }
 
-/* ---- the collection rewrite of a staged unit (compute_unit<true>) -----------------------------------------
- *     ReplaceAll(ReplaceAll(content, "+operator-builder:collection:field", "+operator-builder:field"), "collectionField", "field")
- * Both replacements are deletions ("collection:" at +18 of the first pattern; "collection" of the second, whose 'F' is
- * lowered).  The patterns overlap neither each other nor themselves, and the first replacement cannot create an
- * occurrence of the second: the text it leaves around its deletion is "+operator-builder:" "field", and the second
- * pattern needs a capital 'F'.  So both are found in the ORIGINAL text (a lowered 'F' must not be seen by the
- * search for the first pattern) and applied in one left-to-right compaction.  A match counts only inside one
- * document (ReplaceAll runs per document).  Bookkeeping lives in the phase A bitmaps (rebuilt by phase A). */
-template <int LEN>
-OBM_HD bool rw_match(const uint8_t *t, const char (&pat)[LEN + 1]) {
-#pragma unroll
-    for (int k = 0; k < LEN; k++) if (t[k] != (uint8_t)pat[k]) return false;
-    return true;
-}
-OBMW_DEV void rw_mark(uint32_t *bm, uint32_t a, uint32_t b) { /* bits [a, b), b - a <= 32 */
-    for (uint32_t w = a >> 5; w <= (b - 1u) >> 5; w++) WATOMIC_OR(&bm[w], range_mask(w << 5, a, b));
-}
-/* compacts W.text[lo_pos, hi_pos) in place and moves W.dstart[0..nd] with it; returns the new hi_pos */
-OBMW_DEV uint32_t rewrite_staged(WarpSmem &W, UnitSet &S, uint32_t nd, uint32_t lo_pos, uint32_t hi_pos) {
-    const uint32_t lane = WLANE();
-    uint32_t *del = S.u.bm.nlw, *low = S.u.bm.spw; /* dropped bytes; lowered 'F's */
-    const uint32_t r0 = lo_pos / ROW, r1 = (hi_pos + ROW - 1) / ROW;
-    for (uint32_t w = r0 * 32u + lane; w < r1 * 32u; w += 32) { del[w] = 0; low[w] = 0; }
-    WSYNC();
-    /* detect: exact SIMD tests for the anchors '+' (first pattern, at +0) and 'F' (second, at +10), then verify */
-    bool any = false;
-    for (uint32_t r = r0; r < r1; r++) {
-        const uint32_t pos0 = r * ROW + lane * 32u;
-        const uint32_t keep = range_mask(pos0, lo_pos, hi_pos);
-        uint32_t plus = 0, eff = 0;
-        if (keep) {
-            const uint4 a = reinterpret_cast<const uint4 *>(W.text + pos0)[0], b = reinterpret_cast<const uint4 *>(W.text + pos0)[1];
-            const uint32_t x[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
-#pragma unroll
-            for (int k = 7; k >= 0; k--) { plus = nib_append(plus, zflag8(x[k] ^ 0x2B2B2B2Bu)); eff = nib_append(eff, zflag8(x[k] ^ 0x46464646u)); }
-            plus &= keep; eff &= keep;
-        }
-        while (plus | eff) {
-            const bool second = plus == 0;
-            const uint32_t q = pos0 + OBMW_FFS(second ? eff : plus) - 1u;
-            if (second) eff &= eff - 1u; else plus &= plus - 1u;
-            if (second && q < lo_pos + 10u) continue;
-            const uint32_t p = second ? q - 10u : q, len = second ? 15u : 34u;
-            if (p + len > hi_pos) continue;
-            if (!(second ? rw_match<15>(W.text + p, "collectionField") : rw_match<34>(W.text + p, "+operator-builder:collection:field"))) continue;
-            uint32_t dlo = 0, dhi = nd; /* the document of p: last d with dstart[d] <= p */
-            while (dhi - dlo > 1) { const uint32_t mid = (dlo + dhi) >> 1; if (W.dstart[mid] <= p) dlo = mid; else dhi = mid; }
-            if (W.dstart[dlo + 1] < p + len) continue; /* cut by a document border */
-            if (second) { rw_mark(del, p, p + 10u); rw_mark(low, p + 10u, p + 11u); }
-            else rw_mark(del, p + 18u, p + 29u);
-            any = true;
-        }
-    }
-    if (!WBALLOT(any)) return hi_pos;
-    /* compact, row by row: every kept byte moves to a position <= its own, and a row's bytes only to positions below the
-     * next row, so "read the row into registers, sync, write it left" is safe */
-    const uint32_t dq = lane <= nd ? W.dstart[lane] : 0u;
-    uint32_t dnew = dq, run = lo_pos;
-    for (uint32_t r = r0; r < r1; r++) {
-        const uint32_t pos0 = r * ROW + lane * 32u;
-        const uint32_t keep = range_mask(pos0, lo_pos, hi_pos);
-        const uint32_t km = keep ? keep & ~del[pos0 >> 5] : 0u, lm = keep ? low[pos0 >> 5] : 0u;
-        const uint32_t c = OBMT_POPC(km);
-        uint32_t incl = c;
-        OBMW_SCAN_INCL(incl);
-        const uint32_t o = run + incl - c; /* new position of the lane's first kept byte */
-        run += WSHFL(incl, 31);
-        /* a document start in this row: the kept bytes before it */
-        const uint32_t src = (dq >> 5) & 31u;
-        const uint32_t o_s = WSHFL(o, src), km_s = WSHFL(km, src);
-        if (lane < nd && dq >= r * ROW && dq < (r + 1) * ROW) dnew = o_s + OBMT_POPC(km_s & ((1u << (dq & 31u)) - 1u));
-        const uint4 a = reinterpret_cast<const uint4 *>(W.text + pos0)[0], b = reinterpret_cast<const uint4 *>(W.text + pos0)[1];
-        const uint32_t x[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
-        WSYNC();
-        if (km && !(km == keep && o == pos0 + OBMW_FFS(keep) - 1u)) { /* not already in place */
-            uint32_t at = o;
-#pragma unroll
-            for (uint32_t k = 0; k < 32; k++) {
-                if ((km >> k) & 1u) {
-                    uint32_t v = (x[k >> 2] >> (8u * (k & 3u))) & 0xFFu;
-                    if ((lm >> k) & 1u) v = 'f';
-                    W.text[at++] = (uint8_t)v;
-                }
-            }
-        }
-        WSYNC();
-    }
-    if (lane <= nd) W.dstart[lane] = (lane == nd || dq >= hi_pos) ? run : dnew; /* trailing empty documents start at the end */
-    WSYNC();
-    return run;
-}
-
 /* ---- first half of a unit: stage its text, scan it, assemble the tuple positions ---- */
-template <bool REWRITE = false, class Hooks>
+template <class Hooks>
 OBMW_DEV void compute_unit(WarpSmem &W, UnitSet &S, const WArgs &A, const obm::Tables &T, Hooks &H, const UnitDesc &D, bool prestaged, UnitRegs &R OBMW_PC_PARAM) {
     const uint32_t lane = WLANE();
     const uint32_t u = D.u, da = D.da, nd = D.db - D.da, extra = D.extra;
@@ -574,13 +472,7 @@ OBMW_DEV void compute_unit(WarpSmem &W, UnitSet &S, const WArgs &A, const obm::T
         if (lane < nd) W.dflag[lane] = 0;
         WSYNC();
         H.stage_wait(W, load);
-        OBMW_PC_MARK(PC_STAGE); /* the rewrite of k_warp_scan<true> counts as phase A */
-        if constexpr (REWRITE) hi_pos = rewrite_staged(W, S, nd, lo_pos, hi_pos);
-    }
-    uint64_t nbytes = 0;
-    if constexpr (REWRITE) { /* the byte chain gets the unit's count a whole scan ahead of write_text's resolve */
-        nbytes = (uint64_t)(hi_pos - lo_pos) + (extra ? A.lg_off[da + nd + 1] - A.lg_off[da + nd] : 0ull);
-        H.publish_bytes(u, nbytes);
+        OBMW_PC_MARK(PC_STAGE);
     }
     /* one scan of the whole range; when it has more owning lines than the owner table holds (lines of a few bytes) the
      * same call site then counts it document by document (write_unit scans each document again when it writes it) */
@@ -620,41 +512,7 @@ OBMW_DEV void compute_unit(WarpSmem &W, UnitSet &S, const WArgs &A, const obm::T
     }
     R.extra = extra;
     if (extra) R.total += A.counts[da + nd];
-    if constexpr (REWRITE) { R.kept = hi_pos - lo_pos; R.nbytes = nbytes; }
 }
-
-/* ---- compute_unit<true>'s rewritten text and its document offsets at their final place (base = rewritten bytes of all
- * earlier units); the caller writes before the text dies (the next unit's bulk copy).  Only A.out_bytes, which is
- * 16-byte aligned, is written, and only inside [base, base + nbytes). ---- */
-OBMW_DEV void write_text(const WarpSmem &W, const WArgs &A, const UnitRegs &R, uint64_t base) {
-    const uint32_t lane = WLANE();
-    const uint32_t nd = R.nd, n = R.kept;
-    if (nd) {
-        const uint32_t lo = W.dstart[0];
-        if (lane <= nd) A.out_doc_off[R.da + lane] = base + (W.dstart[lane] - lo);
-        uint32_t head = (uint32_t)((16u - (base & 15u)) & 15u);
-        if (head > n) head = n;
-        if (lane < head) A.out_bytes[base + lane] = W.text[lo + lane];
-        const uint32_t nq = (n - head) >> 4;
-        const uint32_t *tw = reinterpret_cast<const uint32_t *>(W.text);
-        uint4 *dst = reinterpret_cast<uint4 *>(A.out_bytes + base + head); /* 16-byte aligned */
-        for (uint32_t k = lane; k < nq; k += 32) { /* 16 output bytes from five shared-memory words (the staging buffer has room behind the text) */
-            const uint32_t s = lo + head + 16u * k, wq = s >> 2, sh = (s & 3u) * 8u;
-            const uint32_t a0 = tw[wq], a1 = tw[wq + 1], a2 = tw[wq + 2], a3 = tw[wq + 3], a4 = tw[wq + 4];
-            uint4 v;
-            v.x = OBMW_FUNNEL_R(a0, a1, sh); v.y = OBMW_FUNNEL_R(a1, a2, sh); v.z = OBMW_FUNNEL_R(a2, a3, sh); v.w = OBMW_FUNNEL_R(a3, a4, sh);
-            dst[k] = v;
-        }
-        const uint32_t t0 = head + 16u * nq;
-        if (lane < n - t0) A.out_bytes[base + t0 + lane] = W.text[lo + t0 + lane];
-    }
-    if (R.extra && lane == 0) { /* the tile's large document follows the unit's small ones (its text: after the scan) */
-        if (nd == 0) A.out_doc_off[R.da] = base;
-        A.out_doc_off[R.da + nd + 1] = base + R.nbytes;
-    }
-    WSYNC(); /* the reads of W.text precede the next bulk copy into it */
-}
-
 
 /* ---- deferred path: the unit's tuples packed into W.fin in final order (only units without needs_text) -------
  * Returns false when the unit does not fit (more than FIN_CAP tuples, a line number beyond the packed form): the

@@ -173,9 +173,9 @@ class Scanner:
 
     def lex_collection_batch_device(self, d_bytes, d_doc_off, ndocs, total_bytes, d_out_bytes, out_bytes_cap, d_out_doc_off, d_out, out_cap,
                                     d_tuple_off, d_status=None, d_counts=None, stream=None):
-        """lex_batch_device of a collection batch with Manifest.LoadContent's rewrite fused in (include/obmarkers.h:
+        """Manifest.LoadContent's rewrite of a collection batch, then lex_batch_device of the result (include/obmarkers.h:
         obm_lex_collection_batch_device): writes the rewritten bytes (d_out_bytes, 16-byte aligned, out_bytes_cap >=
-        total_bytes) and their offsets, and the tuples of the rewritten documents. Asynchronous."""
+        total_bytes) and their offsets, and the tuples of the rewritten documents. Synchronises the stream."""
         self._check(self._L.obm_lex_collection_batch_device(self._h, d_bytes, d_doc_off, ndocs, total_bytes, d_out_bytes, out_bytes_cap,
                                                             d_out_doc_off, d_out, out_cap, d_tuple_off, d_status, d_counts, stream))
 

@@ -1,17 +1,13 @@
-"""obm_lex_collection_batch_device: Manifest.LoadContent's collection rewrite (manifests/manifest.go:89-95) fused into the
-warp scan.  Its outputs must equal the composition obm_rewrite_collection_markers_device -> obm_lex_batch_device bit for
-bit, and the lexemes must equal the oracle's over the documents rewritten by Python's bytes.replace (Go's ReplaceAll).
-
-CPU: the device source of the collection variant (compute_unit<true> + write_text) replayed on the host by 32 fibers per
-warp (tests/hostsim/collection.cpp), against the Python rewrite followed by the host lexer.  GPU: the library itself."""
+"""obm_lex_collection_batch_device: Manifest.LoadContent's collection rewrite (manifests/manifest.go:89-95) followed by the
+warp scan of its result.  Its outputs must equal, bit for bit, the two calls it is defined as,
+obm_rewrite_collection_markers_device -> obm_lex_batch_device, and the lexemes must equal the oracle's over the documents
+rewritten by Python's bytes.replace (Go's ReplaceAll).  All on the GPU."""
 import random
 
 import numpy as np
 import pytest
 
 from tests import corpus_util as cu
-from tests import hostsim
-from tests.hostsim import collection as hs_collection
 
 P1, P2 = b"+operator-builder:collection:field", b"collectionField"
 TILE, ROW, MAXDOC = 12288, 1024, 13296  # obm_warp.h: a unit's tile, phase A's row, the largest document a unit holds
@@ -79,7 +75,8 @@ def corpus_units():
 
 
 def corpus_large():
-    """documents above MAXDOC: rewritten on the large path; one shrinks below MAXDOC, two are adjacent"""
+    """documents above MAXDOC, the largest document a unit of the warp scan holds; one shrinks below MAXDOC when
+    rewritten, two are adjacent"""
     line = b"  - item  # " + P1 + b":name=a.b,type=int,default=3\n"
     big = (line + b"key: value\n") * 400
     shrink = (b"# " + P1 + b"\n") * (MAXDOC // 36 + 2)
@@ -87,50 +84,8 @@ def corpus_large():
     return [b"k: v # " + P1 + b":name=x\n", big, shrink, b"", big[:20000], b"collectionField\n", P2 * 1000, b"tail " + P1 + b"\n"]
 
 
-CPU_CORPORA = {"fixtures": corpus_fixtures, "flavour1": corpus_flavour1, "patterns": corpus_patterns, "shifts": corpus_shifts,
-               "units": corpus_units, "large": corpus_large}
-
-
-# ---- CPU: the host replay of the collection variant ----------------------------------------------------------------
-def check_host(docs, skew=0):
-    out_bytes, out_off, tuples, toff, _stats = hs_collection.collection_batch(docs, skew)
-    want = [rewrite(d) for d in docs]
-    end = int(out_off[-1])
-    assert end == sum(len(w) for w in want)
-    assert out_bytes[end:end + 16] == b"\xee" * 16, "bytes written past the rewritten batch"
-    for i, w in enumerate(want):
-        assert out_bytes[int(out_off[i]):int(out_off[i + 1])] == w, (i, docs[i][:80])
-        got = tuples[int(toff[i]):int(toff[i + 1])]
-        exp = hostsim.lex_doc(w)
-        assert len(got) == len(exp) and np.array_equal(got, exp), (i, docs[i][:80], hostsim.fmt_tuples(got)[:20], hostsim.fmt_tuples(exp)[:20])
-    assert int(toff[-1]) == len(tuples)
-
-
-@pytest.mark.parametrize("name", sorted(CPU_CORPORA))
-def test_host_collection_variant(name):
-    docs = CPU_CORPORA[name]()
-    assert docs
-    for skew in (0, 5):
-        check_host(docs, skew)
-
-
-def test_host_collection_variant_rewrites_something():
-    docs = corpus_flavour1(8)
-    assert sum(rewrite(d) != d for d in docs) == 8  # the collection spelling: every document has patterns
-
-
-def test_host_stale_shared_memory_between_units():
-    """a batch of long units, then short ones: what the long ones left in the warp's buffer must not matter (the replay
-    keeps its shared memory across calls, like a persistent warp across units)"""
-    long_docs = [(b"# " + P1 + b":name=a\n" + b"+" * 200 + b"\n") * 50]
-    check_host(long_docs)
-    check_host([b"k: v\n", P2[:12], b"# +x:y=1\n", b"collectionFiel", b"", b"+operator-builder:collection:fiel"])
-    check_host(long_docs + [b"# " + P2] * 3)
-
-
-def test_host_empty_batch():
-    out_bytes, out_off, tuples, toff, _ = hs_collection.collection_batch([])
-    assert len(tuples) == 0 and int(out_off[0]) == 0 and int(toff[0]) == 0
+CORPORA = {"fixtures": corpus_fixtures, "flavour1": corpus_flavour1, "patterns": corpus_patterns, "shifts": corpus_shifts,
+           "units": corpus_units, "large": corpus_large}
 
 
 # ---- GPU: the library -------------------------------------------------------------------------------------------------
@@ -155,7 +110,7 @@ def _outputs(n_bytes, ndocs, cap):
                 counts=torch.full((2,), -1, dtype=torch.int64, device="cuda:0"))
 
 
-def _fused(sc, d_bytes, d_off, ndocs, total, o, cap, mode=0):
+def _call(sc, d_bytes, d_off, ndocs, total, o, cap, mode=0):
     import torch
     old = sc.set_mode(mode)
     try:
@@ -190,33 +145,30 @@ def _same(a, b, status_words=(0, 1, 2, 3)):
 
 
 def compare_on_device(sc, oracle, docs, byte_shift=0, cap=None, with_oracle=True):
-    """fused (mode 0) == composition in mode 0 == the fused call in mode 1 (which runs the composition with the exact
+    """the call (mode 0) == the two calls made explicitly in mode 0 == the call in mode 1 (whose scan is the exact
     lexer); then the lexemes against the oracle over the Python-rewritten documents"""
     import operator_builder_b200 as ob
     d_bytes, d_off, off = _dev(docs, byte_shift)
     ndocs, total = len(docs), int(off[-1])
     cap = cap if cap is not None else 2 * total + 2 * ndocs + 16
-    fused = _outputs(total, ndocs, cap)
-    _fused(sc, d_bytes, d_off, ndocs, total, fused, cap)
+    call = _outputs(total, ndocs, cap)
+    _call(sc, d_bytes, d_off, ndocs, total, call, cap)
     comp = _outputs(total, ndocs, cap)
     _composition(sc, d_bytes, d_off, ndocs, total, comp, cap)
-    # status[1] counts the documents the exact lexer took: a document above MAXDOC takes the large path in the fused call
-    # even when its rewritten text is shorter, while the composition lexes the rewritten text line-parallel
-    shrinks = any(len(d) > MAXDOC >= len(rewrite(d)) for d in docs)
-    _same(fused, comp, status_words=(0, 2, 3) if shrinks else (0, 1, 2, 3))
+    _same(call, comp)
     exact = _outputs(total, ndocs, cap)
-    _fused(sc, d_bytes, d_off, ndocs, total, exact, cap, mode=1)
-    _same(fused, exact, status_words=(0, 2))  # status[1] counts the documents the exact lexer took: all of them in mode 1
+    _call(sc, d_bytes, d_off, ndocs, total, exact, cap, mode=1)
+    _same(call, exact, status_words=(0, 2))  # status[1] counts the documents the exact lexer took: all of them in mode 1
     want = [rewrite(d) for d in docs]
-    noff = fused["doc_off"].cpu().numpy()
-    out_bytes = fused["bytes"].cpu().numpy().tobytes()
+    noff = call["doc_off"].cpu().numpy()
+    out_bytes = call["bytes"].cpu().numpy().tobytes()
     assert int(noff[-1]) == sum(len(w) for w in want)
     assert out_bytes[int(noff[-1]):] == b"\xee" * (len(out_bytes) - int(noff[-1])), "bytes written past out_doc_off[ndocs]"
     for i, w in enumerate(want):
         assert out_bytes[int(noff[i]):int(noff[i + 1])] == w, (i, docs[i][:80])
-    if with_oracle and int(fused["status"][0].item()) == 0:
-        tuples = fused["out"].cpu().numpy().view(np.uint64)
-        toff = fused["toff"].cpu().numpy().view(np.uint64)
+    if with_oracle and int(call["status"][0].item()) == 0:
+        tuples = call["out"].cpu().numpy().view(np.uint64)
+        toff = call["toff"].cpu().numpy().view(np.uint64)
         wdata = np.frombuffer(b"".join(want) + b"\0", dtype=np.uint8)[:-1]
         woff = np.zeros(ndocs + 1, dtype=np.uint64)
         woff[1:] = np.cumsum([len(w) for w in want]) if want else []
@@ -224,7 +176,7 @@ def compare_on_device(sc, oracle, docs, byte_shift=0, cap=None, with_oracle=True
         for i, w in enumerate(want):
             got = ob.decode_doc_raw(w, tuples[int(toff[i]):int(toff[i + 1])])
             assert got == want_stream[int(want_off[i]):int(want_off[i + 1])], (i, docs[i][:80])
-    return fused
+    return call
 
 
 @pytest.fixture(scope="module")
@@ -236,9 +188,9 @@ def scanner():
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("name", sorted(CPU_CORPORA))
+@pytest.mark.parametrize("name", sorted(CORPORA))
 def test_device_fused_equals_composition(scanner, oracle, name):
-    compare_on_device(scanner, oracle, CPU_CORPORA[name]())
+    compare_on_device(scanner, oracle, CORPORA[name]())
 
 
 @pytest.mark.gpu
@@ -270,9 +222,9 @@ def test_device_no_documents(scanner, oracle):
 @pytest.mark.gpu
 def test_device_tuple_capacity(scanner, oracle):
     """out_cap too small: status[0] as for obm_lex_batch_device, nothing written past out_cap; the bytes are complete"""
-    fused = compare_on_device(scanner, oracle, corpus_flavour1(200), cap=1000, with_oracle=False)
-    assert int(fused["status"][0].item()) == 1
-    assert bool((fused["out"][1000:] == -1).all())
+    call = compare_on_device(scanner, oracle, corpus_flavour1(200), cap=1000, with_oracle=False)
+    assert int(call["status"][0].item()) == 1
+    assert bool((call["out"][1000:] == -1).all())
 
 
 @pytest.mark.gpu
@@ -296,8 +248,8 @@ def test_device_bad_arguments(scanner):
 
 @pytest.mark.gpu
 def test_device_full_size_c3(scanner, oracle):
-    """C3 at full size (1,048,576 x 4 KiB, flavour 1, generated on the device): fused == composition on the device, and the
-    per-document hash of the fused stream over the rewritten bytes == the oracle's over the same bytes"""
+    """C3 at full size (1,048,576 x 4 KiB, flavour 1, generated on the device): the call == the two calls made explicitly, and
+    the per-document hash of its tuple stream over the rewritten bytes == the oracle's over the same bytes"""
     import os
     import torch
     from operator_builder_b200 import _native
@@ -311,26 +263,26 @@ def test_device_full_size_c3(scanner, oracle):
     d_off = torch.empty(ndocs + 1, dtype=torch.int64, device="cuda:0")
     scanner.generate_corpus_device(d_bytes.data_ptr(), d_off.data_ptr(), ndocs, doc_bytes, 0, 1, st)
     cap = total // 16
-    fused = _outputs(total, ndocs, cap)
-    _fused(scanner, d_bytes, d_off, ndocs, total, fused, cap)
+    call = _outputs(total, ndocs, cap)
+    _call(scanner, d_bytes, d_off, ndocs, total, call, cap)
     comp = _outputs(total, ndocs, cap)
     _composition(scanner, d_bytes, d_off, ndocs, total, comp, cap)
-    _same(fused, comp)
+    _same(call, comp)
     del comp
     torch.cuda.empty_cache()
-    assert int(fused["status"][0].item()) == 0 and int(fused["counts"][0].item()) == 8 * ndocs
+    assert int(call["status"][0].item()) == 0 and int(call["counts"][0].item()) == 8 * ndocs
     d_hash = torch.zeros(ndocs, dtype=torch.int64, device="cuda:0")
     d_nhost = torch.zeros(1, dtype=torch.int32, device="cuda:0")
-    rc = _native.lib().obm_hash_batch_device(scanner.handle, fused["bytes"].data_ptr(), fused["doc_off"].data_ptr(), ndocs, fused["out"].data_ptr(),
-                                             fused["toff"].data_ptr(), d_hash.data_ptr(), d_nhost.data_ptr(), st)
+    rc = _native.lib().obm_hash_batch_device(scanner.handle, call["bytes"].data_ptr(), call["doc_off"].data_ptr(), ndocs, call["out"].data_ptr(),
+                                             call["toff"].data_ptr(), d_hash.data_ptr(), d_nhost.data_ptr(), st)
     assert rc == 0
     torch.cuda.synchronize()
     assert int(d_nhost.item()) == 0
     got = d_hash.cpu().numpy().view(np.uint64)
-    noff = fused["doc_off"].cpu().numpy().astype(np.uint64)
-    host = fused["bytes"][:int(noff[-1])].cpu().numpy()
+    noff = call["doc_off"].cpu().numpy().astype(np.uint64)
+    host = call["bytes"][:int(noff[-1])].cpu().numpy()
     assert int(noff[-1]) < total  # the collection spelling shrinks
-    del fused, d_bytes
+    del call, d_bytes
     torch.cuda.empty_cache()
     threads = max(1, len(os.sched_getaffinity(0)))
     _n_lex, n_mark, _h, want = oracle.scan_batch(host, noff, threads, want_doc_hash=True)

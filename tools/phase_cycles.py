@@ -1,5 +1,5 @@
 #!/usr/bin/env python3
-"""Where k_warp_scan<false>'s cycles go: per-phase cycle accounting of the fused warp kernel on the bench corpus
+"""Where k_warp_scan's cycles go: per-phase cycle accounting of the fused warp kernel on the bench corpus
 (configs[3], 4 KiB manifests generated on the device, HBM resident; 2 GiB by default, OBM_PHASE_DOCS documents).
 
 Needs the phase-clock build of the library (libobmarkers_phase.so, compiled with -DOBMW_PHASE_CLOCKS; __graft_entry__.build()
