@@ -369,6 +369,32 @@ int64_t obm_results_format_doc(const obm_registry *reg, const uint8_t *doc, uint
                                uint8_t **out, uint64_t *out_len);
 int64_t obm_parse_doc(const obm_registry *reg, const uint8_t *doc, uint64_t doc_len, const obm_tuple *tuples, uint64_t ntuples,
                       uint8_t **out, uint64_t *out_len);
+/*
+ * Parse a packed batch held in HOST memory on the device: H2D, the scan, obm_parse_batch_device and the D2H of the
+ * records only -- the tuple stream stays on the device except for the documents the host must parse itself.
+ *   results / args   exactly what obm_parse_batch_device writes for the same batch with doc_base = 0: `doc` is the
+ *                    document index in this batch, arg_base indexes `args` as a whole, spans are document-relative.
+ *                    Document d's Results are results[doc_res_off[d] .. doc_res_off[d+1]).
+ *   host_tuples      for every document whose one record is OBM_R_HOST, its whole tuple stream (as obm_lex_batch returns
+ *                    it) in host_tuples[doc_host_off[d] .. doc_host_off[d+1]); that range is empty for every other
+ *                    document.  So for every d,
+ *                        obm_results_format_doc(reg, doc_d, len_d, host_tuples + doc_host_off[d], doc_host_off[d+1] - doc_host_off[d],
+ *                                               results + doc_res_off[d], doc_res_off[d+1] - doc_res_off[d], args, ...)
+ *                    gives obm_parse_doc's bytes for that document.
+ *   totals           [3]: results, args, fallback tuples.
+ * Capacities as in obm_lex_batch: NULL or 0 capacities size the buffers; when any total exceeds its capacity the call
+ * returns OBM_E_CAPACITY with totals, doc_res_off and doc_host_off (ndocs+1 each) filled, and writes nothing past any
+ * capacity (the arrays' contents are then unspecified).  The registry is limited as for the device parser (8 markers, 64
+ * arguments, 1024 bytes of names), else OBM_E_ARG; doc_off is checked as by obm_lex_batch; ndocs = 0 is valid.
+ * obm_set_mode applies to the scan (a scratch overflow redoes the chunk in mode 1, as obm_lex_batch does), and batches of
+ * at least two chunks (obm_set_chunk_bytes) are pipelined over obm_lex_batch's three streams.  stats: the scan counters,
+ * bytes, ms_kernels = scan + parse + gather (summed over chunks), ms_total.  obm_launches_last_call counts every kernel of
+ * the call, over all its chunks.
+ */
+int obm_parse_batch(obm_handle *h, const obm_registry *reg, const uint8_t *bytes, const uint64_t *doc_off, uint32_t ndocs,
+                    obm_result *results, uint64_t res_cap, obm_arg *args, uint64_t arg_cap, uint64_t *doc_res_off /* ndocs+1 */,
+                    obm_tuple *host_tuples, uint64_t host_cap, uint64_t *doc_host_off /* ndocs+1 */,
+                    uint64_t *totals /* [3]: results, args, host tuples */, obm_stats *stats);
 
 #ifdef __cplusplus
 }

@@ -8,4 +8,5 @@ directory name is what the project brief prescribes; operator_builder_b200.py al
 from ._native import NativeError, SO_PATH  # noqa: F401
 from .lexer import (BatchResult, Lexeme, LexemeType, Lexer, Position, Scanner, ZERO_LEXEME,  # noqa: F401
                     decode_doc_raw, generate_corpus_host, Registry, parse_doc_raw, Comm,
-                    FIELD_MARKER, COLLECTION_MARKER, RESOURCE_MARKER)
+                    FIELD_MARKER, COLLECTION_MARKER, RESOURCE_MARKER, ParseBatchResult, RESULT_DT, ARG_DT,
+                    results_format_doc)

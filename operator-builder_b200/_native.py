@@ -16,6 +16,7 @@ EXPORTS = [
     "obm_comm_unique_id", "obm_comm_create", "obm_comm_destroy", "obm_lex_batch_sharded_device",
     "obm_registry_free", "obm_registry_define", "obm_parse_doc", "obm_hash_batch_device", "obm_parse_batch_device", "obm_results_format_doc", "obm_marker_index_device",
     "obm_marker_index_flat_device", "obm_rewrite_collection_markers_device", "obm_split_docs_device", "obm_lex_collection_batch_device",
+    "obm_parse_batch",
 ]
 
 
@@ -87,6 +88,10 @@ def lib():
     L.obm_lex_collection_batch_device.argtypes = [vp, vp, vp, u32, u64, vp, u64, vp, vp, u64, vp, vp, vp, vp]
     L.obm_marker_index_device.argtypes = [vp, vp, vp, vp, u32, vp, vp, vp, u64, vp, vp]
     L.obm_parse_batch_device.argtypes = [vp, vp, vp, vp, u32, u32, vp, vp, vp, u64, vp, u64, vp, vp, vp]
+    L.obm_parse_batch.argtypes = [vp, vp, vp, vp, u32, vp, u64, vp, u64, vp, vp, u64, vp, vp, ctypes.POINTER(ObmStats)]
+    L.obm_results_format_doc.argtypes = [vp, ctypes.c_char_p, u64, vp, u64, vp, u64, vp, ctypes.POINTER(ctypes.POINTER(ctypes.c_uint8)),
+                                         ctypes.POINTER(u64)]
+    L.obm_results_format_doc.restype = ctypes.c_int64
     L.obm_hash_batch_device.argtypes = [vp, vp, vp, u32, vp, vp, vp, vp, vp]
     L.obm_comm_unique_id.argtypes = [vp]
     L.obm_comm_create.argtypes = [vp, vp, ctypes.c_int, ctypes.c_int, ctypes.POINTER(vp)]

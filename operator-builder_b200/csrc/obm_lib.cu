@@ -383,15 +383,26 @@ struct obm_handle {
     /* obm_lex_batch pipelines large host batches in chunks over three slots: H2D of chunk k+1, scan of
      * chunk k and D2H of chunk k-1 overlap (each slot has its own stream, staging and scratch) */
     struct Slot {
-        cudaStream_t st; cudaEvent_t ev_scan; cudaEvent_t ev_k0, ev_k1; /* around the chunk's scan kernels (timing) */
+        cudaStream_t st; cudaEvent_t ev_scan; cudaEvent_t ev_k0, ev_k1; /* around the chunk's scan kernels (timing); obm_parse_batch
+                                                                            records them again around parse + gather */
         uint8_t *d_bytes; uint64_t d_bytes_cap;
         uint64_t *d_doc_off; uint64_t d_doc_off_cap;
         uint64_t *d_tuple_off; uint64_t d_tuple_off_cap;
         obm_tuple *d_out; uint64_t d_out_cap;
         void *scratch; uint64_t scratch_bytes;
         uint32_t *d_status; unsigned long long *d_counts;
+        /* obm_parse_batch: the chunk's records, offsets, fallback tuples and {results, args} totals */
+        obm_result *d_res; uint64_t d_res_cap;
+        obm_arg *d_args; uint64_t d_args_cap;
+        uint64_t *d_res_off; uint64_t d_res_off_cap;
+        uint64_t *d_host_off; uint64_t d_host_off_cap;
+        obm_tuple *d_host; uint64_t d_host_cap;
+        uint32_t *d_host_cnt; uint64_t d_host_cnt_cap;
+        uint64_t *d_host_sums; uint64_t d_host_sums_cap;
+        uint64_t *d_ptot; uint64_t d_ptot_cap;
         uint64_t *h_doc_off; uint64_t h_doc_off_cap; /* pinned: rebased offsets of the chunk */
-        uint64_t *h_info;                             /* pinned: [0] total, [1..2] status words, [3..4] counts */
+        uint64_t *h_info;                             /* pinned: [0] total, [1..2] status words, [3..4] counts,
+                                                         obm_parse_batch: [5..7] results, args, fallback tuples */
         uint32_t d0, d1; uint64_t b0; bool busy;
     } slots[3];
     bool slots_ready;
@@ -459,6 +470,8 @@ extern "C" void obm_destroy(obm_handle *h) {
         cudaStreamSynchronize(sl.st);
         cudaFree(sl.d_bytes); cudaFree(sl.d_doc_off); cudaFree(sl.d_tuple_off); cudaFree(sl.d_out); cudaFree(sl.scratch);
         cudaFree(sl.d_status); cudaFree(sl.d_counts); cudaFreeHost(sl.h_doc_off); cudaFreeHost(sl.h_info);
+        cudaFree(sl.d_res); cudaFree(sl.d_args); cudaFree(sl.d_res_off); cudaFree(sl.d_host_off); cudaFree(sl.d_host);
+        cudaFree(sl.d_host_cnt); cudaFree(sl.d_host_sums); cudaFree(sl.d_ptot);
         cudaEventDestroy(sl.ev_scan); cudaEventDestroy(sl.ev_k0); cudaEventDestroy(sl.ev_k1); cudaStreamDestroy(sl.st);
     }
     for (int i = 0; i < 4; i++) cudaEventDestroy(h->ev[i]);
@@ -801,6 +814,21 @@ static int slots_init(obm_handle *h) {
     return OBM_OK;
 }
 
+/* enqueue the scan of the slot's staged chunk (nb bytes) + the D2H of its info words */
+static int chunk_scan(obm_handle *h, obm_handle::Slot &sl, uint64_t nb, bool want_out) {
+    const uint32_t nd = sl.d1 - sl.d0;
+    OBM_CUDA(h, cudaEventRecord(sl.ev_k0, sl.st));
+    int rc = lex_device_impl(h, sl.d_bytes, sl.d_doc_off, nd, nb, want_out ? sl.d_out : nullptr, want_out ? sl.d_out_cap : 0, sl.d_tuple_off,
+                             sl.d_status, sl.d_counts, sl.st, &sl.scratch, &sl.scratch_bytes);
+    if (rc != OBM_OK) return rc;
+    OBM_CUDA(h, cudaEventRecord(sl.ev_k1, sl.st));
+    OBM_CUDA(h, cudaMemcpyAsync(&sl.h_info[0], sl.d_tuple_off + nd, 8, cudaMemcpyDeviceToHost, sl.st));
+    OBM_CUDA(h, cudaMemcpyAsync(&sl.h_info[1], sl.d_status, 16, cudaMemcpyDeviceToHost, sl.st));
+    OBM_CUDA(h, cudaMemcpyAsync(&sl.h_info[3], sl.d_counts, 16, cudaMemcpyDeviceToHost, sl.st));
+    OBM_CUDA(h, cudaEventRecord(sl.ev_scan, sl.st));
+    return OBM_OK;
+}
+
 /* enqueue H2D + scan + info D2H of documents [d0, d1) on slot sl */
 static int chunk_issue(obm_handle *h, obm_handle::Slot &sl, const uint8_t *bytes, const uint64_t *doc_off, uint32_t d0, uint32_t d1,
                        bool want_out) {
@@ -822,17 +850,8 @@ static int chunk_issue(obm_handle *h, obm_handle::Slot &sl, const uint8_t *bytes
     for (uint32_t d = 0; d <= nd; d++) sl.h_doc_off[d] = doc_off[d0 + d] - b0;
     OBM_CUDA(h, cudaMemcpyAsync(sl.d_doc_off, sl.h_doc_off, ((uint64_t)nd + 1) * 8, cudaMemcpyHostToDevice, sl.st));
     if (nb) OBM_CUDA(h, cudaMemcpyAsync(sl.d_bytes, bytes + b0, nb, cudaMemcpyHostToDevice, sl.st));
-    OBM_CUDA(h, cudaEventRecord(sl.ev_k0, sl.st));
-    rc = lex_device_impl(h, sl.d_bytes, sl.d_doc_off, nd, nb, want_out ? sl.d_out : nullptr, want_out ? sl.d_out_cap : 0, sl.d_tuple_off,
-                         sl.d_status, sl.d_counts, sl.st, &sl.scratch, &sl.scratch_bytes);
-    if (rc != OBM_OK) return rc;
-    OBM_CUDA(h, cudaEventRecord(sl.ev_k1, sl.st));
-    OBM_CUDA(h, cudaMemcpyAsync(&sl.h_info[0], sl.d_tuple_off + nd, 8, cudaMemcpyDeviceToHost, sl.st));
-    OBM_CUDA(h, cudaMemcpyAsync(&sl.h_info[1], sl.d_status, 16, cudaMemcpyDeviceToHost, sl.st));
-    OBM_CUDA(h, cudaMemcpyAsync(&sl.h_info[3], sl.d_counts, 16, cudaMemcpyDeviceToHost, sl.st));
-    OBM_CUDA(h, cudaEventRecord(sl.ev_scan, sl.st));
     sl.d0 = d0; sl.d1 = d1; sl.b0 = b0; sl.busy = true;
-    return OBM_OK;
+    return chunk_scan(h, sl, nb, want_out);
 }
 
 struct ChunkTotals { uint64_t tuples, markers, lexemes, exact, fatal; bool overflow, need_exact; float ms_kernels; };
@@ -857,6 +876,38 @@ static int chunk_retire(obm_handle *h, obm_handle::Slot &sl, obm_tuple *out, uin
     return OBM_OK;
 }
 
+/* chunk boundaries (document aligned: a chunk ends before the first document that would take it past chunk_bytes, and
+ * holds at least one document) and the per-chunk base for the final offset fix-up; malloc'd, NULL when out of memory */
+struct Ck { uint32_t d0, d1; uint64_t base; };
+static Ck *cut_chunks(const uint64_t *doc_off, uint32_t ndocs, uint64_t chunk_bytes, uint32_t *nck) {
+    Ck *cks = nullptr; uint32_t n = 0, capck = 0;
+    for (uint32_t d = 0; d < ndocs;) {
+        uint32_t e = d; const uint64_t lim = doc_off[d] + chunk_bytes;
+        while (e < ndocs && (doc_off[e + 1] <= lim || e == d)) e++;
+        if (n == capck) {
+            capck = capck ? capck * 2 : 64;
+            Ck *g = (Ck *)realloc(cks, capck * sizeof(Ck));
+            if (!g) { free(cks); return nullptr; }
+            cks = g;
+        }
+        cks[n++] = Ck{d, e, 0};
+        d = e;
+    }
+    if (!cks) cks = (Ck *)malloc(sizeof(Ck));
+    *nck = n;
+    return cks;
+}
+
+/* the host entry points' checks of a packed batch: ascending offsets, documents within OBM_MAX_DOC_BYTES, bytes given */
+static int check_host_batch(obm_handle *h, const uint8_t *bytes, const uint64_t *doc_off, uint32_t ndocs) {
+    for (uint32_t d = 0; d < ndocs; d++) {
+        if (doc_off[d + 1] < doc_off[d]) { set_err(h, "doc_off is not ascending at document %u", d); return OBM_E_ARG; }
+        if (doc_off[d + 1] - doc_off[d] > OBM_MAX_DOC_BYTES) { set_err(h, "document %u exceeds %llu bytes", d, (unsigned long long)OBM_MAX_DOC_BYTES); return OBM_E_ARG; }
+    }
+    if (doc_off[ndocs] > doc_off[0] && !bytes) { set_err(h, "bytes is NULL"); return OBM_E_ARG; }
+    return OBM_OK;
+}
+
 /* returns 1 when the batch was handled here, 0 to let the caller use the single-shot path, <0 on error */
 static int lex_batch_chunked(obm_handle *h, const uint8_t *bytes, const uint64_t *doc_off, uint32_t ndocs, obm_tuple *out, uint64_t out_cap,
                              uint64_t *out_count, uint64_t *doc_tuple_off, obm_stats *stats, int *result) {
@@ -867,16 +918,9 @@ static int lex_batch_chunked(obm_handle *h, const uint8_t *bytes, const uint64_t
     if ((rc = slots_init(h)) != OBM_OK) return rc;
     OBM_CUDA(h, cudaEventRecord(h->ev[0], h->stream));
     ChunkTotals T = {0, 0, 0, 0, 0, false, false, 0.f};
-    /* chunk boundaries (document aligned) and the per-chunk tuple base for the final offset fix-up */
-    struct Ck { uint32_t d0, d1; uint64_t base; };
-    Ck *cks = nullptr; uint32_t nck = 0, capck = 0;
-    for (uint32_t d = 0; d < ndocs;) {
-        uint32_t e = d; const uint64_t lim = doc_off[d] + chunk_bytes;
-        while (e < ndocs && (doc_off[e + 1] <= lim || e == d)) e++;
-        if (nck == capck) { capck = capck ? capck * 2 : 64; cks = (Ck *)realloc(cks, capck * sizeof(Ck)); if (!cks) return OBM_E_NOMEM; }
-        cks[nck++] = Ck{d, e, 0};
-        d = e;
-    }
+    uint32_t nck = 0;
+    Ck *cks = cut_chunks(doc_off, ndocs, chunk_bytes, &nck);
+    if (!cks) return OBM_E_NOMEM;
     int err = OBM_OK;
     for (uint32_t k = 0; k < nck + 2 && err == OBM_OK; k++) {
         if (k < nck) {
@@ -918,15 +962,11 @@ extern "C" int obm_lex_batch(obm_handle *h, const uint8_t *bytes, const uint64_t
                              obm_stats *stats) {
     if (!h) return OBM_E_ARG;
     if (!doc_off || !out_count || !doc_tuple_off) { set_err(h, "doc_off, out_count and doc_tuple_off must not be NULL"); return OBM_E_ARG; }
+    int rc;
+    if ((rc = check_host_batch(h, bytes, doc_off, ndocs)) != OBM_OK) return rc;
     uint64_t total = doc_off[ndocs] - doc_off[0];
-    for (uint32_t d = 0; d < ndocs; d++) {
-        if (doc_off[d + 1] < doc_off[d]) { set_err(h, "doc_off is not ascending at document %u", d); return OBM_E_ARG; }
-        if (doc_off[d + 1] - doc_off[d] > OBM_MAX_DOC_BYTES) { set_err(h, "document %u exceeds %llu bytes", d, (unsigned long long)OBM_MAX_DOC_BYTES); return OBM_E_ARG; }
-    }
-    if (total && !bytes) { set_err(h, "bytes is NULL"); return OBM_E_ARG; }
     OBM_CUDA(h, cudaSetDevice(h->device));
     cudaStream_t st = h->stream;
-    int rc;
     {
         int result = OBM_OK;
         rc = lex_batch_chunked(h, bytes, doc_off, ndocs, out, out_cap, out_count, doc_tuple_off, stats, &result);
@@ -1673,22 +1713,19 @@ extern "C" int obm_hash_batch_device(obm_handle *h, const void *d_bytes, const v
     return OBM_OK;
 }
 
-extern "C" int obm_parse_batch_device(obm_handle *h, const obm_registry *reg, const void *d_bytes, const void *d_doc_off, uint32_t ndocs, uint32_t doc_base,
-                                      const void *d_tuples, const void *d_doc_tuple_off, void *d_results, uint64_t res_cap, void *d_args, uint64_t arg_cap,
-                                      void *d_doc_res_off, void *d_totals, void *stream) {
-    if (!h || !reg || !d_doc_off || !d_doc_tuple_off || !d_doc_res_off) return OBM_E_ARG;
-    obmr::DevTypedRegistry R;
-    if (!obm_registry_flatten(reg, &R)) { set_err(h, "registry too large for the device parser (8 markers, 64 arguments, 1024 bytes of names)"); return OBM_E_ARG; }
-    OBM_CUDA(h, cudaSetDevice(h->device));
-    cudaStream_t st = (cudaStream_t)stream;
+/* obm_parse_batch_device on a flattened registry and the given scratch (the handle's, or a chunk slot's); *launches = kernels */
+static int parse_device_impl(obm_handle *h, const obmr::DevTypedRegistry &R, const void *d_bytes, const void *d_doc_off, uint32_t ndocs, uint32_t doc_base,
+                             const void *d_tuples, const void *d_doc_tuple_off, void *d_results, uint64_t res_cap, void *d_args, uint64_t arg_cap,
+                             void *d_doc_res_off, void *d_totals, cudaStream_t st, void **scratch_p, uint64_t *scratch_bytes_p, uint32_t *launches) {
+    *launches = 0;
     uint64_t *roff = (uint64_t *)d_doc_res_off;
     if (ndocs == 0) { OBM_CUDA(h, cudaMemsetAsync(roff, 0, 8, st)); if (d_totals) OBM_CUDA(h, cudaMemsetAsync(d_totals, 0, 16, st)); return OBM_OK; }
     const uint64_t need = 2 * align_up((uint64_t)ndocs * 4 + 4, 256) + align_up(((uint64_t)ndocs + 1) * 8, 256) + align_up((uint64_t)scan_tiles(ndocs) * 8 + 8, 256);
-    if (h->scratch_bytes < need) {
-        if (h->scratch) { OBM_CUDA(h, cudaStreamSynchronize(st)); cudaFree(h->scratch); h->scratch = nullptr; h->scratch_bytes = 0; }
-        OBM_CUDA(h, cudaMalloc(&h->scratch, need)); h->scratch_bytes = need;
+    if (*scratch_bytes_p < need) {
+        if (*scratch_p) { OBM_CUDA(h, cudaStreamSynchronize(st)); cudaFree(*scratch_p); *scratch_p = nullptr; *scratch_bytes_p = 0; }
+        OBM_CUDA(h, cudaMalloc(scratch_p, need)); *scratch_bytes_p = need;
     }
-    uint8_t *q = (uint8_t *)h->scratch;
+    uint8_t *q = (uint8_t *)*scratch_p;
     uint32_t *cres = (uint32_t *)q; q += align_up((uint64_t)ndocs * 4 + 4, 256);
     uint32_t *carg = (uint32_t *)q; q += align_up((uint64_t)ndocs * 4 + 4, 256);
     uint64_t *aoff = (uint64_t *)q; q += align_up(((uint64_t)ndocs + 1) * 8, 256);
@@ -1722,7 +1759,184 @@ extern "C" int obm_parse_batch_device(obm_handle *h, const obm_registry *reg, co
                                                       (const uint64_t *)d_doc_tuple_off, RN, cres, carg, roff, aoff, (obm_result *)d_results, res_cap,
                                                       (obm_arg *)d_args, arg_cap);
     OBM_CUDA(h, cudaGetLastError());
+    *launches = 7 + ((d_results && d_args) ? 1 : 0);
     return OBM_OK;
+}
+
+static bool flatten_for_device(obm_handle *h, const obm_registry *reg, obmr::DevTypedRegistry *R) {
+    if (obm_registry_flatten(reg, R)) return true;
+    set_err(h, "registry too large for the device parser (8 markers, 64 arguments, 1024 bytes of names)");
+    return false;
+}
+
+extern "C" int obm_parse_batch_device(obm_handle *h, const obm_registry *reg, const void *d_bytes, const void *d_doc_off, uint32_t ndocs, uint32_t doc_base,
+                                      const void *d_tuples, const void *d_doc_tuple_off, void *d_results, uint64_t res_cap, void *d_args, uint64_t arg_cap,
+                                      void *d_doc_res_off, void *d_totals, void *stream) {
+    if (!h || !reg || !d_doc_off || !d_doc_tuple_off || !d_doc_res_off) return OBM_E_ARG;
+    obmr::DevTypedRegistry R;
+    if (!flatten_for_device(h, reg, &R)) return OBM_E_ARG;
+    OBM_CUDA(h, cudaSetDevice(h->device));
+    uint32_t launches;
+    return parse_device_impl(h, R, d_bytes, d_doc_off, ndocs, doc_base, d_tuples, d_doc_tuple_off, d_results, res_cap, d_args, arg_cap, d_doc_res_off,
+                             d_totals, (cudaStream_t)stream, &h->scratch, &h->scratch_bytes, &launches);
+}
+
+/* ------------------------------------------------------------------------------------------- */
+/* obm_parse_batch: host batches through the slot pipeline of obm_lex_batch with the parser behind the scan; a chunk's   */
+/* tuples stay on the device, only records, offsets and fallback tuples are copied back (obm_parse_gather.cuh)         */
+/* ------------------------------------------------------------------------------------------- */
+#include "obm_parse_gather.cuh"
+
+struct ParseTotals { uint64_t res, args, host; uint32_t launches; };
+
+static uint32_t grid_for(uint64_t items, uint32_t per_block) {
+    const uint64_t g = (items + per_block - 1) / per_block;
+    return (uint32_t)(g < 1 ? 1 : g > 8192 ? 8192 : g);
+}
+
+/* After the slot's scan: redo it while its result is unusable -- scratch overflow (the exact kernels, mode 1, as
+ * obm_lex_batch does) or more tuples than the slot's buffer holds (grown to the count) -- then enqueue the parse, the
+ * fallback gather and the D2H of the chunk's totals.  The record buffers are sized from the chunk's tuple count, which
+ * bounds them: every Result and every argument belongs to a distinct tuple of its document (the walk writes one Result
+ * per MarkerEnd, error or OBM_R_HOST tuple, one argument per value tuple), and fallback tuples are a subset. */
+static int parse_chunk(obm_handle *h, obm_handle::Slot &sl, const obmr::DevTypedRegistry &R, ChunkTotals &T, ParseTotals &P) {
+    const uint32_t nd = sl.d1 - sl.d0;
+    const uint64_t nb = sl.h_doc_off[nd];
+    int mode = h->mode, rc;
+    for (;;) {
+        OBM_CUDA(h, cudaEventSynchronize(sl.ev_scan));
+        const uint32_t *stw = (const uint32_t *)&sl.h_info[1];
+        if (stw[ST_RESERVED] && mode != 1) mode = 1;
+        else if (sl.h_info[0] > sl.d_out_cap) { if ((rc = ensure(h, &sl.d_out, &sl.d_out_cap, sl.h_info[0])) != OBM_OK) return rc; }
+        else break;
+        const int saved = h->mode;
+        h->mode = mode;
+        rc = chunk_scan(h, sl, nb, true);
+        h->mode = saved;
+        if (rc != OBM_OK) return rc;
+        P.launches += h->launches;
+    }
+    { float ms = 0.f; if (cudaEventElapsedTime(&ms, sl.ev_k0, sl.ev_k1) == cudaSuccess) T.ms_kernels += ms; }
+    const uint32_t *stw = (const uint32_t *)&sl.h_info[1];
+    const uint64_t ntup = sl.h_info[0];
+    T.tuples += ntup; T.markers += sl.h_info[3]; T.lexemes += sl.h_info[4]; T.exact += stw[ST_DOCS_EXACT]; T.fatal += stw[ST_DOCS_FATAL];
+    if ((rc = ensure(h, &sl.d_res, &sl.d_res_cap, ntup)) != OBM_OK) return rc;
+    if ((rc = ensure(h, &sl.d_args, &sl.d_args_cap, ntup)) != OBM_OK) return rc;
+    if ((rc = ensure(h, &sl.d_host, &sl.d_host_cap, ntup)) != OBM_OK) return rc;
+    if ((rc = ensure(h, &sl.d_res_off, &sl.d_res_off_cap, (uint64_t)nd + 1)) != OBM_OK) return rc;
+    if ((rc = ensure(h, &sl.d_host_off, &sl.d_host_off_cap, (uint64_t)nd + 1)) != OBM_OK) return rc;
+    if ((rc = ensure(h, &sl.d_host_cnt, &sl.d_host_cnt_cap, (uint64_t)nd + 1)) != OBM_OK) return rc;
+    if ((rc = ensure(h, &sl.d_host_sums, &sl.d_host_sums_cap, (uint64_t)scan_tiles(nd) + 1)) != OBM_OK) return rc;
+    if ((rc = ensure(h, &sl.d_ptot, &sl.d_ptot_cap, 2)) != OBM_OK) return rc;
+    OBM_CUDA(h, cudaEventRecord(sl.ev_k0, sl.st));
+    uint32_t pl = 0;
+    rc = parse_device_impl(h, R, sl.d_bytes, sl.d_doc_off, nd, sl.d0, sl.d_out, sl.d_tuple_off, sl.d_res, sl.d_res_cap, sl.d_args, sl.d_args_cap,
+                           sl.d_res_off, sl.d_ptot, sl.st, &sl.scratch, &sl.scratch_bytes, &pl);
+    if (rc != OBM_OK) return rc;
+    const uint32_t nt = scan_tiles(nd);
+    obmg::k_fallback_counts<<<grid_for(nd, obmg::THREADS), obmg::THREADS, 0, sl.st>>>(sl.d_res, sl.d_res_off, sl.d_tuple_off, nd, sl.d_host_cnt);
+    k_scan_tiles<<<nt, SCAN_THREADS, 0, sl.st>>>(sl.d_host_cnt, nd, sl.d_host_off, sl.d_host_sums);
+    k_scan_sums<<<1, SCAN_THREADS, 0, sl.st>>>(sl.d_host_sums, nt, sl.d_host_off + nd);
+    k_scan_add<<<nt, SCAN_THREADS, 0, sl.st>>>(sl.d_host_off, nd, sl.d_host_sums, ~0ull, nullptr);
+    obmg::k_fallback_gather<<<grid_for(nd, obmg::THREADS / 32), obmg::THREADS, 0, sl.st>>>(sl.d_out, sl.d_tuple_off, sl.d_host_off, nd, sl.d_host);
+    OBM_CUDA(h, cudaGetLastError());
+    P.launches += pl + 5;
+    OBM_CUDA(h, cudaEventRecord(sl.ev_k1, sl.st));
+    OBM_CUDA(h, cudaMemcpyAsync(&sl.h_info[5], sl.d_ptot, 16, cudaMemcpyDeviceToHost, sl.st));
+    OBM_CUDA(h, cudaMemcpyAsync(&sl.h_info[7], sl.d_host_off + nd, 8, cudaMemcpyDeviceToHost, sl.st));
+    OBM_CUDA(h, cudaEventRecord(sl.ev_scan, sl.st));
+    return OBM_OK;
+}
+
+struct ParseOut {
+    obm_result *results; uint64_t res_cap; obm_arg *args; uint64_t arg_cap; uint64_t *doc_res_off;
+    obm_tuple *host_tuples; uint64_t host_cap; uint64_t *doc_host_off;
+};
+
+/* wait for the slot's parse, rebase its records and offsets by the totals of the chunks before it, and enqueue their D2H
+ * at the final host positions; an array whose running total passes its capacity is not copied from there on */
+static int parse_retire(obm_handle *h, obm_handle::Slot &sl, const ParseOut &O, ChunkTotals &T, ParseTotals &P) {
+    OBM_CUDA(h, cudaEventSynchronize(sl.ev_scan));
+    { float ms = 0.f; if (cudaEventElapsedTime(&ms, sl.ev_k0, sl.ev_k1) == cudaSuccess) T.ms_kernels += ms; }
+    const uint32_t nd = sl.d1 - sl.d0;
+    const uint64_t nres = sl.h_info[5], nargs = sl.h_info[6], nhost = sl.h_info[7];
+    if (P.res || P.args || P.host) {
+        obmg::k_rebase_records<<<grid_for(nres > nd ? nres : nd, obmg::THREADS), obmg::THREADS, 0, sl.st>>>(
+            sl.d_res, nres, (uint32_t)P.args, sl.d_res_off, P.res, sl.d_host_off, P.host, nd);
+        OBM_CUDA(h, cudaGetLastError());
+        P.launches += 1;
+    }
+    OBM_CUDA(h, cudaMemcpyAsync(O.doc_res_off + sl.d0, sl.d_res_off, (uint64_t)nd * 8, cudaMemcpyDeviceToHost, sl.st));
+    OBM_CUDA(h, cudaMemcpyAsync(O.doc_host_off + sl.d0, sl.d_host_off, (uint64_t)nd * 8, cudaMemcpyDeviceToHost, sl.st));
+    if (O.results && nres && P.res + nres <= O.res_cap)
+        OBM_CUDA(h, cudaMemcpyAsync(O.results + P.res, sl.d_res, nres * sizeof(obm_result), cudaMemcpyDeviceToHost, sl.st));
+    if (O.args && nargs && P.args + nargs <= O.arg_cap)
+        OBM_CUDA(h, cudaMemcpyAsync(O.args + P.args, sl.d_args, nargs * sizeof(obm_arg), cudaMemcpyDeviceToHost, sl.st));
+    if (O.host_tuples && nhost && P.host + nhost <= O.host_cap)
+        OBM_CUDA(h, cudaMemcpyAsync(O.host_tuples + P.host, sl.d_host, nhost * sizeof(obm_tuple), cudaMemcpyDeviceToHost, sl.st));
+    P.res += nres; P.args += nargs; P.host += nhost;
+    sl.busy = false;
+    return OBM_OK;
+}
+
+extern "C" int obm_parse_batch(obm_handle *h, const obm_registry *reg, const uint8_t *bytes, const uint64_t *doc_off, uint32_t ndocs,
+                               obm_result *results, uint64_t res_cap, obm_arg *args, uint64_t arg_cap, uint64_t *doc_res_off,
+                               obm_tuple *host_tuples, uint64_t host_cap, uint64_t *doc_host_off, uint64_t *totals, obm_stats *stats) {
+    if (!h) return OBM_E_ARG;
+    if (!reg || !doc_off || !doc_res_off || !doc_host_off || !totals) {
+        set_err(h, "reg, doc_off, doc_res_off, doc_host_off and totals must not be NULL"); return OBM_E_ARG;
+    }
+    int rc;
+    if ((rc = check_host_batch(h, bytes, doc_off, ndocs)) != OBM_OK) return rc;
+    obmr::DevTypedRegistry R;
+    if (!flatten_for_device(h, reg, &R)) return OBM_E_ARG;
+    OBM_CUDA(h, cudaSetDevice(h->device));
+    if ((rc = slots_init(h)) != OBM_OK) return rc;
+    const ParseOut O{results, results ? res_cap : 0, args, args ? arg_cap : 0, doc_res_off, host_tuples, host_tuples ? host_cap : 0, doc_host_off};
+    const uint64_t total = doc_off[ndocs] - doc_off[0];
+    OBM_CUDA(h, cudaEventRecord(h->ev[0], h->stream));
+    /* a batch of fewer than two chunks is one chunk: the same code path, without the overlap */
+    const bool one = total < 2 * h->chunk_bytes || ndocs < 4;
+    uint32_t nck = 0;
+    Ck *cks = cut_chunks(doc_off, ndocs, one ? total + 1 : h->chunk_bytes, &nck);
+    if (!cks) return OBM_E_NOMEM;
+    ChunkTotals T = {0, 0, 0, 0, 0, false, false, 0.f};
+    ParseTotals P = {0, 0, 0, 0};
+    int err = OBM_OK;
+    /* iteration k: issue chunk k (H2D + scan), parse chunk k-1, retire chunk k-2 */
+    for (uint32_t k = 0; k < nck + 2 && err == OBM_OK; k++) {
+        if (k < nck) {
+            obm_handle::Slot &sl = h->slots[k % 3];
+            if (k >= 3) { cudaError_t e_ = cudaStreamSynchronize(sl.st); if (e_ != cudaSuccess) { set_err(h, "cudaStreamSynchronize failed: %s", cudaGetErrorString(e_)); err = OBM_E_CUDA; break; } }
+            if ((err = chunk_issue(h, sl, bytes, doc_off, cks[k].d0, cks[k].d1, true)) != OBM_OK) break;
+            P.launches += h->launches;
+        }
+        if (k >= 1 && k - 1 < nck && (err = parse_chunk(h, h->slots[(k - 1) % 3], R, T, P)) != OBM_OK) break;
+        if (k >= 2 && k - 2 < nck) err = parse_retire(h, h->slots[(k - 2) % 3], O, T, P);
+    }
+    for (auto &sl : h->slots) cudaStreamSynchronize(sl.st);
+    free(cks);
+    if (err != OBM_OK) return err;
+    doc_res_off[ndocs] = P.res; doc_host_off[ndocs] = P.host;
+    totals[0] = P.res; totals[1] = P.args; totals[2] = P.host;
+    h->launches = P.launches;
+    int result = OBM_OK;
+    if (P.res > O.res_cap || P.args > O.arg_cap || P.host > O.host_cap) {
+        set_err(h, "capacity too small: %llu results (cap %llu), %llu args (cap %llu), %llu fallback tuples (cap %llu)",
+                (unsigned long long)P.res, (unsigned long long)O.res_cap, (unsigned long long)P.args, (unsigned long long)O.arg_cap,
+                (unsigned long long)P.host, (unsigned long long)O.host_cap);
+        result = OBM_E_CAPACITY;
+    }
+    OBM_CUDA(h, cudaEventRecord(h->ev[3], h->stream));
+    OBM_CUDA(h, cudaStreamSynchronize(h->stream));
+    if (stats) {
+        memset(stats, 0, sizeof *stats);
+        stats->n_tuples = T.tuples; stats->n_markers = T.markers; stats->n_lexemes = T.lexemes;
+        stats->n_docs_exact = T.exact; stats->n_docs_fatal = T.fatal; stats->bytes = total;
+        cudaEventElapsedTime(&stats->ms_total, h->ev[0], h->ev[3]);
+        stats->ms_kernels = T.ms_kernels; /* scan + parse + gather, summed over the chunks */
+    }
+    return result;
 }
 
 #include "obm_rewrite.cuh"

@@ -8,6 +8,9 @@ Reference today: one parser -- one lexer goroutine -- per YAML node, over Head +
     gpu     ONE Scanner.lex_batch over all of them
     pass 2  walk again in the same order; visit k parses the pre-lexed stream k (the parser is unchanged)
 
+inspect_manifests_parsed does the same with ONE Scanner.parse_batch (scan and parser on the device): visit k formats the
+Result records of input k.
+
 What yaml.v3 attaches to which node as Head / Line / Foot comment is outside this path (it stays Go on the host, and no
 reference test pins it): callers hand in the node tree with its comment strings.
 """
@@ -64,8 +67,8 @@ def collect(docs: Sequence[Node]) -> Collected:
     return Collected(list(docs), inputs)
 
 
-def inspect_manifests_batched(scanner: Scanner, registry: Registry, manifests: Sequence[Sequence[Node]]):
-    """-> per manifest: list of (serialised parser Results of one visit, group) in visiting order.  One GPU call in all."""
+def _pack(manifests: Sequence[Sequence[Node]]):
+    """pass 1 over every manifest -> (collected, index of each manifest's first input, inputs, packed bytes, offsets)"""
     collected = [collect(m) for m in manifests]
     first, inputs = [], []
     for c in collected:
@@ -75,18 +78,35 @@ def inspect_manifests_batched(scanner: Scanner, registry: Registry, manifests: S
     off = np.zeros(len(inputs) + 1, dtype=np.uint64)
     if inputs:
         off[1:] = np.cumsum([len(x) for x in inputs])
-    res = scanner.lex_batch(data, off)
+    return collected, first, inputs, data, off
+
+
+def _per_visit(collected, first, results_of):
+    """pass 2: per manifest, (results_of(k), group) for visit k in visiting order"""
     out = []
     for c, k0 in zip(collected, first):
         k = [k0]
         per = []
 
         def one(group, node, k=k, per=per):
-            i = k[0]
-            t = res.tuples[int(res.doc_tuple_off[i]):int(res.doc_tuple_off[i + 1])]
-            per.append((parse_doc_raw(registry, inputs[i], t), group))
+            per.append((results_of(k[0]), group))
             k[0] += 1
 
         visit(c.docs, one)
         out.append(per)
     return out
+
+
+def inspect_manifests_batched(scanner: Scanner, registry: Registry, manifests: Sequence[Sequence[Node]]):
+    """-> per manifest: list of (serialised parser Results of one visit, group) in visiting order.  One GPU call in all."""
+    collected, first, inputs, data, off = _pack(manifests)
+    res = scanner.lex_batch(data, off)
+    return _per_visit(collected, first, lambda i: parse_doc_raw(registry, inputs[i], res.tuples[int(res.doc_tuple_off[i]):int(res.doc_tuple_off[i + 1])]))
+
+
+def inspect_manifests_parsed(scanner: Scanner, registry: Registry, manifests: Sequence[Sequence[Node]]):
+    """inspect_manifests_batched's result from ONE Scanner.parse_batch: the parser runs on the device too, and the host only
+    formats the Result records (and parses the few nodes whose record says R_HOST from their returned tuples)."""
+    collected, first, inputs, data, off = _pack(manifests)
+    res = scanner.parse_batch(registry, data, off)
+    return _per_visit(collected, first, lambda i: res.format_doc(i, inputs[i]))

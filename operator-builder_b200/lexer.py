@@ -165,6 +165,35 @@ class Scanner:
         stats = {f: getattr(st, f) for f, _ in ObmStats._fields_}
         return BatchResult(out[:cnt.value], toff, stats)
 
+    def parse_batch(self, registry: "Registry", data, doc_off, res_cap: int = None, arg_cap: int = None,
+                    host_cap: int = None) -> "ParseBatchResult":
+        """The parser over a host batch in one device call (include/obmarkers.h: obm_parse_batch): H2D, scan, parse, and
+        back only the Result records plus the tuples of the documents the host must parse itself.  Without capacities a
+        sizing call comes first; with them, too small a capacity raises NativeError (OBM_E_CAPACITY)."""
+        buf = np.frombuffer(data, dtype=np.uint8) if not isinstance(data, np.ndarray) else data
+        doc_off = np.ascontiguousarray(doc_off, dtype=np.uint64)
+        ndocs = len(doc_off) - 1
+        roff = np.zeros(ndocs + 1, dtype=np.uint64)
+        hoff = np.zeros(ndocs + 1, dtype=np.uint64)
+        totals = np.zeros(3, dtype=np.uint64)
+        st = ObmStats()
+        if res_cap is None or arg_cap is None or host_cap is None:
+            rc = self._L.obm_parse_batch(self._h, registry.handle, buf.ctypes.data, doc_off.ctypes.data, ndocs, None, 0, None, 0,
+                                         roff.ctypes.data, None, 0, hoff.ctypes.data, totals.ctypes.data, ctypes.byref(st))
+            if rc not in (0, _native.OBM_E_CAPACITY):
+                self._check(rc)
+            res_cap, arg_cap, host_cap = (int(x) for x in totals)
+        res = np.empty(max(res_cap, 1), dtype=RESULT_DT)
+        args = np.empty(max(arg_cap, 1), dtype=ARG_DT)
+        host = np.empty(max(host_cap, 1), dtype=np.uint64)
+        rc = self._L.obm_parse_batch(self._h, registry.handle, buf.ctypes.data, doc_off.ctypes.data, ndocs, res.ctypes.data, res_cap,
+                                     args.ctypes.data, arg_cap, roff.ctypes.data, host.ctypes.data, host_cap, hoff.ctypes.data,
+                                     totals.ctypes.data, ctypes.byref(st))
+        self._check(rc)
+        stats = {f: getattr(st, f) for f, _ in ObmStats._fields_}
+        nres, nargs, nhost = (int(x) for x in totals)
+        return ParseBatchResult(registry, res[:nres], args[:nargs], roff, host[:nhost], hoff, stats)
+
     def lex_batch_device(self, d_bytes, d_doc_off, ndocs, total_bytes, d_out, out_cap, d_tuple_off, d_status=None,
                          d_counts=None, stream=None):
         """Raw device-pointer entry point (ints / torch .data_ptr()). Asynchronous."""
@@ -327,3 +356,48 @@ def parse_doc_raw(registry: Registry, doc: bytes, tuples: np.ndarray) -> bytes:
     data = ctypes.string_at(out, outlen.value)
     L.obm_free(out)
     return data
+
+
+# obm_result / obm_arg (include/obmarkers.h): the records k_parse_docs writes
+RESULT_DT = np.dtype([("doc", "<u4"), ("tuple", "<u4"), ("text_off", "<u4"), ("text_len", "<u4"), ("reg_id", "<u2"), ("nargs", "<u2"),
+                      ("arg_base", "<u4"), ("flags", "<u4"), ("aux", "<u4")])
+ARG_DT = np.dtype([("name_off", "<u4"), ("val_off", "<u4"), ("val_len", "<u4"), ("name_len", "<u2"), ("kind", "u1"), ("flags", "u1")])
+R_OK, R_NL, R_ERR_PARSEBOOL, R_ERR_FLOAT32, R_HOST, R_ERR_SETARG, R_ERR_MISSING, R_PANIC = 1, 2, 4, 8, 16, 32, 64, 128
+A_SYNTHETIC_TRUE, A_SUPERSEDED = 1, 2
+
+
+def results_format_doc(registry: Registry, doc: bytes, tuples: np.ndarray, results: np.ndarray, args: np.ndarray) -> bytes:
+    """One document's records (results: its slice; args: the batch's whole array) -> the byte format of parse_doc_raw.
+    A document whose record is R_HOST is parsed from `tuples` (obm_results_format_doc)."""
+    L = _native.lib()
+    tuples = np.ascontiguousarray(tuples, dtype=np.uint64)
+    results = np.ascontiguousarray(results, dtype=RESULT_DT)
+    args = np.ascontiguousarray(args, dtype=ARG_DT)
+    out = ctypes.POINTER(ctypes.c_uint8)()
+    outlen = ctypes.c_uint64()
+    n = L.obm_results_format_doc(registry.handle, doc, len(doc), tuples.ctypes.data, len(tuples), results.ctypes.data, len(results),
+                                 args.ctypes.data if len(args) else None, ctypes.byref(out), ctypes.byref(outlen))
+    if n < 0:
+        raise NativeError(n, "obm_results_format_doc")
+    data = ctypes.string_at(out, outlen.value)
+    L.obm_free(out)
+    return data
+
+
+class ParseBatchResult(NamedTuple):
+    """What Scanner.parse_batch returns: document d's Results are results[doc_res_off[d]:doc_res_off[d+1]] (their arg_base
+    indexes `args` as a whole); its tuples are host_tuples[doc_host_off[d]:doc_host_off[d+1]], present only when its one
+    record is R_HOST."""
+    registry: Registry
+    results: np.ndarray       # RESULT_DT[n_results]
+    args: np.ndarray          # ARG_DT[n_args]
+    doc_res_off: np.ndarray   # uint64[ndocs+1]
+    host_tuples: np.ndarray   # uint64[n_fallback_tuples]
+    doc_host_off: np.ndarray  # uint64[ndocs+1]
+    stats: dict
+
+    def format_doc(self, d: int, doc: bytes) -> bytes:
+        """document d's Results in parse_doc_raw's byte format (doc: its bytes)"""
+        r = self.results[int(self.doc_res_off[d]):int(self.doc_res_off[d + 1])]
+        t = self.host_tuples[int(self.doc_host_off[d]):int(self.doc_host_off[d + 1])]
+        return results_format_doc(self.registry, doc, t, r, self.args)
