@@ -44,7 +44,10 @@ extern "C" {
  * pseudo-tuples the host decoder folds away so that the decoded stream is byte-identical to the
  * reference's (Type, Value, Pos) sequence, including its implementation artefacts:
  *   PART    text that sits in the reference lexer's `buffer` without having been emitted; it is
- *           prepended to the Value of the next real lexeme (emit.go:8-17 clears buffer only on emit)
+ *           prepended to the Value of the next real lexeme (emit.go:8-17 clears buffer only on emit).
+ *           A slice longer than OBM_MAX_LEN is sent as PART pieces of OBM_MAX_LEN followed by the rest:
+ *           before a lexeme, a warning, or an ERR_FLOAT / ERR_INT (whose literal is the chain plus its
+ *           own slice, its column taken from off + len)
  *   FLUSH   the reference called flush() (discard.go:68-71; state.go:81,128)
  *   DRIFT   the second backup() of state.go:79/126 shortened the column by one (position.go:44-45)
  *   LINE    position basis: off = byte offset of column 1, len = line number (low 27 bits);

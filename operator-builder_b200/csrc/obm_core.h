@@ -268,7 +268,10 @@ struct NoAccel {
 };
 
 /* ASCII = true: the caller guarantees every byte of the document is < 0x80 (tile path); rune decoding,
- * the Unicode tables and the U+FFFD over-discard drop out at compile time. */
+ * the Unicode tables and the U+FFFD over-discard drop out at compile time.
+ * SHORT = true: the lexer only sees documents of at most 16 KiB (the tile, pipeline and warp kernels), so no
+ * slice can reach OBM_MAX_LEN.  Lexers that may see larger documents (the exact path, the chunk-parallel
+ * large path) keep SHORT = false and send every long slice as PART pieces. */
 
 /* peek.go:65-89 for one ASCII token `tok[0..t)` at offset p of doc d[0..n): on success returns true and
  * sets `width` (= l.width after the final peekN: whitespace BYTES + token bytes). */
@@ -319,7 +322,7 @@ __device__ __forceinline__ Quad src_ldq(const ShBytes &d, uint32_t off16) {
 }
 #endif
 
-template <class Sink, class Accel = NoAccel, bool ASCII = false, class Src = const uint8_t *>
+template <class Sink, class Accel = NoAccel, bool ASCII = false, class Src = const uint8_t *, bool SHORT = false>
 struct Lexer {
     const Tables &T;
     Src d; uint32_t n;
@@ -355,9 +358,10 @@ struct Lexer {
     OBM_HD void sync_start() { s = p; line_s = line_p; base_s = base_p; }
     /* a slice longer than OBM_MAX_LEN is sent as PART pieces.  Inline on purpose: an out-of-line helper taking the
      * sink by reference would force the sink (and its counters) out of registers into local memory for EVERY put.
-     * The ASCII instantiation only sees tile-path documents (<= 16 KiB): the loop vanishes at compile time. */
+     * In the SHORT ASCII instantiations (the hot lexers of the tile and warp kernels) the loop vanishes at compile
+     * time; the SHORT Unicode ones keep it here, where it always was, but not in numeric_error. */
     OBM_HD void put_long_prefix(uint32_t &off, uint32_t &len) {
-        if (!ASCII) while (len > OBM_MAX_LEN) { out.put(OBM_K_PART, off, OBM_MAX_LEN); off += OBM_MAX_LEN; len -= OBM_MAX_LEN; }
+        if (!(ASCII && SHORT)) while (len > OBM_MAX_LEN) { out.put(OBM_K_PART, off, OBM_MAX_LEN); off += OBM_MAX_LEN; len -= OBM_MAX_LEN; }
     }
     /* un-emitted text doc[s,p) becomes a PART (kept in the decoder's pending buffer) */
     OBM_HD void part_tail() {
@@ -384,7 +388,14 @@ struct Lexer {
     OBM_HD void flush() { out.put(OBM_K_FLUSH, p, 0); sync_start(); }
     /* error.go:37-45 (continues in lexComment) / error.go:15-34 (terminates) */
     OBM_HD void located_at_pos(uint32_t kind) { part_tail(); ensure_line(line_p, base_p); out.put(kind, p, 0); }
-    OBM_HD void numeric_error(uint32_t kind) { ensure_line(line_s, base_s); out.put(kind, s, p - s); }
+    /* the literal is quoted in the message and its end p gives the column: a long one goes out as PART pieces and
+     * the error tuple keeps off + len = p */
+    OBM_HD void numeric_error(uint32_t kind) {
+        ensure_line(line_s, base_s);
+        uint32_t off = s, len = p - s;
+        if (!SHORT) put_long_prefix(off, len);
+        out.put(kind, off, len);
+    }
 
     /* ---- reader primitives ---- */
     OBM_HD int peek(uint32_t &w) const {

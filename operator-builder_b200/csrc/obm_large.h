@@ -24,7 +24,9 @@ enum : uint32_t { CF_FATAL = 1, CF_OVERSHOOT = 2 };
 
 OBM_HD uint32_t n_chunks(uint32_t len) { return len == 0 ? 1u : (uint32_t)(((uint64_t)len + LCHUNK - 1) / LCHUNK); }
 
-/* start of chunk c: the first line start (0, or the byte after a '\n') at or after c * LCHUNK; n if there is none.
+/* start of chunk c, looked for inside the chunk only: the first line start (0, or the byte after a '\n') in
+ * [c * LCHUNK, min((c + 1) * LCHUNK, n)], or n if the chunk holds none (resolve_chunk_starts then gives it the next
+ * chunk's start).  Reading one chunk per call keeps the whole search linear in the document, however long its lines.
  * nl_skipped: newlines in [c * LCHUNK, start) */
 OBM_HD uint32_t chunk_start(const uint8_t *doc, uint32_t n, uint32_t c, uint32_t *nl_skipped) {
     *nl_skipped = 0;
@@ -33,10 +35,22 @@ OBM_HD uint32_t chunk_start(const uint8_t *doc, uint32_t n, uint32_t c, uint32_t
     if (nominal >= n) return n;
     uint32_t p = (uint32_t)nominal;
     if (doc[p - 1] == '\n') return p;
-    while (p < n && doc[p] != '\n') p++;
-    if (p >= n) return n;
+    const uint32_t b = (n - p > LCHUNK) ? p + LCHUNK : n;
+    while (p < b && doc[p] != '\n') p++;
+    if (p >= b) return n;
     *nl_skipped = 1;
     return p + 1;
+}
+
+/* After chunk_start for every chunk of a document and line[c] = 1 + newlines before c * LCHUNK + nl_skipped: a chunk
+ * c < nc - 1 with no line start of its own (start beyond its end, i.e. n) takes the start and the line of the next
+ * chunk that has one.  That is the first line start at or after c * LCHUNK, so every chunk that lexes anything keeps
+ * the start and line of a search that runs on past its end; the chunks that take over a start lex nothing. */
+OBM_HD void resolve_chunk_starts(uint32_t *cs, uint32_t *line, uint32_t nc) {
+    for (uint32_t k = nc - 1; k > 1; k--) { /* chunks nc - 2 .. 1, backwards */
+        const uint32_t c = k - 1;
+        if (cs[c] > (uint64_t)k * LCHUNK) { cs[c] = cs[k]; line[c] = line[k]; }
+    }
 }
 
 /* newlines in [c * LCHUNK, min((c + 1) * LCHUNK, n)) */

@@ -181,7 +181,8 @@ k_scan_add(uint64_t *__restrict__ off, uint32_t n, const uint64_t *__restrict__ 
 
 /* ------------------------------------------------------------------------------------------- */
 /* large documents (> obmt::MAXDOC bytes): chunk-parallel exact lexing, see obm_large.h          */
-/* plan (chunks per document, scan) -> prep (chunk starts, newline counts) -> lines -> count ->  */
+/* plan (chunks per document, scan) -> prep (chunk starts, newline counts) -> lines (line numbers; */
+/* a chunk without a line start takes the next one's) -> count ->                                */
 /* resolve (chain check, offsets, or sequential fallback) ... main scan ... -> fill              */
 /* ------------------------------------------------------------------------------------------- */
 struct LargeWs {
@@ -249,6 +250,7 @@ k_large_lines(LargeWs W) {
             const uint32_t sk = W.cline[g0 + c], v = W.cnl[g0 + c];
             W.cline[g0 + c] = 1u + acc + sk; acc += v & 0x7FFFFFFFu; na |= v >> 31;
         }
+        obml::resolve_chunk_starts(W.cs + g0, W.cline + g0, nc);
         W.lch[i] = na ? 0u : 1u; /* reused after the scan: 1 = the document is all ASCII (fast lexer instantiation) */
     }
 }

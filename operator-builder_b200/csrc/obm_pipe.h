@@ -78,7 +78,7 @@ struct LineAccelT {
     }
 };
 typedef LineAccelT<const uint8_t *> LineAccel;
-template <class Src> using GLineLexerT = obm::Lexer<obm::SmallSink, LineAccelT<Src>, true, Src>;
+template <class Src> using GLineLexerT = obm::Lexer<obm::SmallSink, LineAccelT<Src>, true, Src, true>;
 typedef GLineLexerT<const uint8_t *> GLineLexer;
 
 OBM_HD uint32_t plain_count_fwd(item_t it) { return it_line(it) == 1 ? 1u : 2u; }
@@ -155,7 +155,7 @@ OBM_FN item_t k1_owner_item(const SmemScan &S, uint32_t o) {
 
 /* K2: a line of a valid-UTF-8 document that contains bytes >= 0x80: the Unicode lexer in LINE mode from the line
  * start, straight from global memory.  Regular iff it stopped exactly behind this line's newline. */
-typedef obm::Lexer<obm::SmallSink, obm::NoAccel, false> GUniLexer;
+typedef obm::Lexer<obm::SmallSink, obm::NoAccel, false, const uint8_t *, true> GUniLexer;
 OBM_HD_NOINLINE uint32_t k2_unicode_item(const obm::Tables &T, const uint8_t *doc, uint32_t n, item_t it, obm_tuple *out, uint32_t cap,
                                          uint32_t *markers = nullptr, uint32_t *lexemes = nullptr) {
     const uint32_t ls = it_ls(it), line = it_line(it), le = it_line_end(it);

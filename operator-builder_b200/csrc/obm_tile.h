@@ -349,8 +349,8 @@ OBM_FN uint32_t doc_of(const SmemScan &S, uint32_t pos) {
 }
 
 /* The two lexer instantiations the tile kernel carries, each compiled once (noinline). */
-typedef obm::Lexer<obm::SmallSink, BitmapAccel, true> LineLexer;
-typedef obm::Lexer<obm::SmallSink, obm::NoAccel, false> DocLexer;
+typedef obm::Lexer<obm::SmallSink, BitmapAccel, true, const uint8_t *, true> LineLexer;
+typedef obm::Lexer<obm::SmallSink, obm::NoAccel, false, const uint8_t *, true> DocLexer;
 
 /* marker line: LINE mode from the first special.  Sink and lexer live in registers (everything inlines
  * into this one function, which is compiled once and called from the stage and fill phases). */

@@ -48,6 +48,8 @@ def lib():
         L.hs_warp_batch.argtypes = L.hs_tile_batch.argtypes
         L.hs_large_doc.restype = ctypes.c_uint64
         L.hs_large_doc.argtypes = [ctypes.c_char_p, ctypes.c_uint32, ctypes.c_void_p, ctypes.c_uint64, ctypes.POINTER(ctypes.c_uint32)]
+        L.hs_large_chunk_starts.restype = ctypes.c_uint32
+        L.hs_large_chunk_starts.argtypes = [ctypes.c_char_p, ctypes.c_uint32, ctypes.c_void_p, ctypes.c_void_p]
         L.hs_utf8_plain.argtypes = [ctypes.c_char_p, ctypes.c_uint32, ctypes.c_uint32]
         L.hs_parse_float_err.argtypes = [ctypes.c_char_p, ctypes.c_uint32]
         L.hs_atoi_err.argtypes = [ctypes.c_char_p, ctypes.c_uint32]
@@ -81,6 +83,16 @@ def large_doc(doc: bytes):
     n = L.hs_large_doc(doc, len(doc), out.ctypes.data, cap, ctypes.byref(used))
     assert n <= cap
     return out[:n].copy(), bool(used.value)
+
+
+def large_chunk_starts(doc: bytes):
+    """resolved (start, line) of every chunk of the chunk-parallel path -> two numpy uint32 arrays"""
+    L = lib()
+    nc = max(1, -(-len(doc) // 1024))
+    cs = np.zeros(nc, dtype=np.uint32)
+    line = np.zeros(nc, dtype=np.uint32)
+    assert L.hs_large_chunk_starts(doc, len(doc), cs.ctypes.data, line.ctypes.data) == nc
+    return cs, line
 
 
 def decode(doc: bytes, tuples, L=None) -> bytes:

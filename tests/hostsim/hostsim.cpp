@@ -444,12 +444,20 @@ extern "C" uint64_t hs_pipe_batch(const uint8_t *bytes, const uint64_t *doc_off,
  * returns the tuple count; *used_chunks = 1 when the chain validated (no sequential fallback)
  * ------------------------------------------------------------------------------------------- */
 #include "../../operator-builder_b200/csrc/obm_large.h"
+/* k_large_prep + k_large_lines: the resolved start and line of every chunk (cs and line hold n_chunks(n) entries) */
+extern "C" uint32_t hs_large_chunk_starts(const uint8_t *doc, uint32_t n, uint32_t *cs, uint32_t *line) {
+    using namespace obml;
+    const uint32_t nc = n_chunks(n);
+    uint32_t acc = 0;
+    for (uint32_t c = 0; c < nc; c++) { uint32_t sk; cs[c] = chunk_start(doc, n, c, &sk); line[c] = 1 + acc + sk; acc += chunk_newlines(doc, n, c); }
+    resolve_chunk_starts(cs, line, nc);
+    return nc;
+}
 extern "C" uint64_t hs_large_doc(const uint8_t *doc, uint32_t n, obm_tuple *out, uint64_t cap, uint32_t *used_chunks) {
     using namespace obml;
     const uint32_t nc = n_chunks(n);
     std::vector<uint32_t> cs(nc + 1), line(nc), cnt(nc), cend(nc), flag(nc);
-    uint32_t acc = 0;
-    for (uint32_t c = 0; c < nc; c++) { uint32_t sk; cs[c] = chunk_start(doc, n, c, &sk); line[c] = 1 + acc + sk; acc += chunk_newlines(doc, n, c); }
+    hs_large_chunk_starts(doc, n, cs.data(), line.data());
     cs[nc] = n;
     bool valid = true, ascii = true;
     for (uint32_t c = 0; c < nc; c++) ascii = ascii && !chunk_non_ascii(doc, n, c);
