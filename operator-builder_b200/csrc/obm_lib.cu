@@ -674,7 +674,7 @@ static uint64_t warp_scratch_bytes(uint32_t ndocs, uint64_t total_bytes) {
     const uint64_t nt = warp_ntiles(total_bytes), um = warp_units_max(ndocs, total_bytes);
     return align_up((nt + 2) * 4, 256) + align_up((obm_fast_max_large(total_bytes) + 1) * 4, 256) + align_up(nt * 4 + 4, 256) + align_up((nt + 1) * 8, 256) +
            align_up(((uint64_t)scan_tiles((uint32_t)nt) + 1) * 8, 256) + align_up((nt + 1) * sizeof(obmw::WRec), 256) + align_up((um + 1) * 8, 256) +
-           align_up(2 * (um / 32 + 2) * 8, 256) + align_up((um + 1) * 4, 256) + 512;
+           align_up(2 * (um / 32 + 2) * 8, 256) + align_up((um + 1) * sizeof(obmw::WUnit), 256) + 512;
 }
 /* tile index -> (large documents planned and counted on a side stream) units per tile + scan -> k_warp_scan -> fill of
  * the large documents */
@@ -695,11 +695,11 @@ static int obm_warp_launch(obm_handle *h, const uint8_t *d_bytes, const uint64_t
     uint64_t *ubase = (uint64_t *)q; q += up(((uint64_t)ntiles + 1) * 8);
     uint64_t *usums = (uint64_t *)q; q += up(((uint64_t)nt_u + 1) * 8);
     obmw::WRec *wrec = (obmw::WRec *)q; q += up(((uint64_t)ntiles + 1) * sizeof(obmw::WRec));
-    uint32_t *unit_tile = (uint32_t *)q; q += up((um + 1) * 4);
+    obmw::WUnit *units = (obmw::WUnit *)q; q += up((um + 1) * sizeof(obmw::WUnit));
     obmw::WArgs A;
-    A.unit_tile = unit_tile;
+    A.units = units;
     A.bytes = d_bytes; A.doc_off = d_doc_off; A.ndocs = ndocs; A.total_bytes = total_bytes; A.tile_first = tile_first; A.ntiles = ntiles;
-    A.wrec = wrec; A.ubase = ubase;
+    A.ubase = ubase;
     A.st_tuples = (uint64_t *)q; q += up((um + 1) * 8);
     A.st_blocks = (uint64_t *)q; q += up(2 * (um / 32 + 2) * 8); A.units_max = um;
     A.ctl = (uint32_t *)q; /* [0] ticket, [1] n_large */
@@ -717,7 +717,7 @@ static int obm_warp_launch(obm_handle *h, const uint8_t *d_bytes, const uint64_t
     k_scan_tiles<<<nt_u, SCAN_THREADS, 0, st>>>(nun, ntiles, ubase, usums);
     k_scan_sums<<<1, SCAN_THREADS, 0, st>>>(usums, nt_u, ubase + ntiles);
     k_scan_add<<<nt_u, SCAN_THREADS, 0, st>>>(ubase, ntiles, usums, ~0ull, nullptr);
-    obmw::k_wunit_tiles<<<(ntiles + 255) / 256, 256, 0, st>>>(nun, ubase, ntiles, um, unit_tile);
+    obmw::k_wunit_descs<<<(ntiles + 255) / 256, 256, 0, st>>>(d_doc_off, wrec, ubase, ntiles, um, units);
     OBM_CUDA(h, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, obmw::k_warp_scan, (int)(obmw::WPC * 32), smem));
     if (per_sm < 1) per_sm = 1;
     uint32_t grid = (uint32_t)dev_sms * (uint32_t)per_sm; /* persistent warps: a multiple of the SM count */

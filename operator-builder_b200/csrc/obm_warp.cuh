@@ -3,7 +3,7 @@
  *
  *   k_wtile_index   tile -> first document starting in it; list of large documents (> obmw::MAXDOC)
  *   k_wunits        per tile: unit count + record; an exclusive scan gives every unit a static id in document order
- *   k_wunit_tiles   unit -> tile
+ *   k_wunit_descs   unit -> 16-byte descriptor (documents, span and byte offset of its text)
  *   k_warp_scan     persistent warps (no block barrier anywhere): a warp takes a unit by ticket, stages the text of
  *                   each of its units with one TMA bulk copy (cp.async.bulk + mbarrier) into its own slice of shared
  *                   memory and runs obmw::process_unit on it
@@ -44,13 +44,15 @@ k_wtile_index(const uint64_t *__restrict__ doc_off, uint32_t ndocs, uint32_t nti
     if (d < ndocs && doc_off[d + 1] - doc_off[d] > MAXDOC) large_list[atomicAdd(n_large, 1u)] = d;
 }
 
-/* unit -> tile, after the scan of the unit counts */
+/* unit -> descriptor, after the scan of the unit counts */
 __global__ void __launch_bounds__(256)
-k_wunit_tiles(const uint32_t *__restrict__ nunits, const uint64_t *__restrict__ ubase, uint32_t ntiles, uint64_t units_max, uint32_t *__restrict__ unit_tile) {
+k_wunit_descs(const uint64_t *__restrict__ doc_off, const WRec *__restrict__ wrec, const uint64_t *__restrict__ ubase, uint32_t ntiles,
+              uint64_t units_max, WUnit *__restrict__ units) {
     const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
     if (t >= ntiles) return;
+    const WRec r = wrec[t];
     const uint64_t u0 = ubase[t];
-    for (uint32_t k = 0; k < nunits[t] && u0 + k < units_max; k++) unit_tile[u0 + k] = t;
+    for (uint32_t k = 0; k < r.n_units && u0 + k < units_max; k++) units[u0 + k] = make_wunit(doc_off, r, k);
 }
 
 __global__ void __launch_bounds__(256)
@@ -94,11 +96,12 @@ __device__ __forceinline__ uint64_t chain_resolve(uint64_t *st_units, uint64_t *
     const uint32_t lane = threadIdx.x & 31;
     const uint32_t b = u >> 5, r = u & 31;
     volatile uint64_t *st0 = st_units, *blk = st_blocks, *bex = st_blocks + nblocks;
-    uint64_t s;
+    uint64_t s, mine;
     uint32_t backoff = 32; /* ns; doubles up to ~2 us: a thousand warps polling at a fixed short interval saturate L2 and slow the
                             * very warps they wait for (marker-dense units resolve right after publishing) */
-    for (;;) {
+    for (;;) { /* the block's prefix is read in the same round trip as its st0 entries: once flagged, it never changes */
         s = lane < r ? st0[(b << 5) + lane] : LB_AGG;
+        mine = b ? bex[b] : BEX_FLAG;
         if (__ballot_sync(0xffffffffu, (s >> 62) == 0) == 0) break;
         __nanosleep(backoff); if (backoff < 2048) backoff <<= 1;
     }
@@ -106,7 +109,6 @@ __device__ __forceinline__ uint64_t chain_resolve(uint64_t *st_units, uint64_t *
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) partial += __shfl_xor_sync(0xffffffffu, partial, o);
     uint64_t P = 0;
-    const uint64_t mine = b ? bex[b] : BEX_FLAG;
     if (mine & BEX_FLAG) P = mine & ~BEX_FLAG;
     else {
         int64_t hi = (int64_t)b - 1; /* nearest block not yet accounted for */
@@ -152,17 +154,17 @@ k_warp_scan(WArgs A) {
     /* unit iterator: UNITS by ticket, in document order (not tiles: a warp that held two units of one tile would publish
      * the second only after writing the first, and with units that resolve right after publishing that serialises the
      * whole chain).  The ticket after next is taken while this unit is processed, and the NEXT unit's descriptor
-     * (document offsets -> source address of its text) is ready one unit ahead */
+     * (one 16-byte load) is requested before this unit is scanned, so that it arrives under the scan */
     uint32_t tn = 0;
-    auto next_unit = [&]() -> UnitDesc {
-        const uint32_t u = __shfl_sync(0xffffffffu, tn, 0);
-        if (u >= nunits) { UnitDesc d{0, 0, 0, 0, 0, 0, 0, false}; return d; }
+    auto take_unit = [&](uint32_t &u, WUnit &w) {
+        u = __shfl_sync(0xffffffffu, tn, 0);
+        if (u >= nunits) return;
         if (lane == 0) tn = atomicAdd(&A.ctl[WC_TICKET], 1u);
-        const uint32_t t = A.unit_tile[u];
-        const WRec rec = A.wrec[t];
-        uint32_t da, db, extra;
-        wrec_unit(rec, u - (uint32_t)A.ubase[t], da, db, extra);
-        return make_desc(A, u, da, db, extra);
+        w = A.units[u];
+    };
+    auto unit_desc = [&](uint32_t u, const WUnit &w) -> UnitDesc {
+        if (u >= nunits) { UnitDesc d{0, 0, 0, 0, 0, 0, 0, false, 0}; return d; }
+        return make_desc(A, u, w);
     };
     if (lane == 0) tn = atomicAdd(&A.ctl[WC_TICKET], 1u);
 #ifdef OBMW_PHASE_CLOCKS
@@ -170,17 +172,25 @@ k_warp_scan(WArgs A) {
     pc.t0 = (uint32_t)clock64();
     uint32_t pc_units = 0;
 #endif
-    UnitDesc cur = next_unit();
+    uint32_t un = 0; WUnit wn{0, 0, 0};
+    take_unit(un, wn);
+    UnitDesc cur = unit_desc(un, wn);
     bool prestaged = false;
     while (cur.valid) {
-        const UnitDesc nxt = next_unit();
+        take_unit(un, wn);
         OBMW_PC_MARK(PC_OTHER);
         UnitRegs R;
         compute_unit(S, S.set, A, T, H, cur, prestaged, R OBMW_PC_ARG);
         chain_publish(A.st_tuples, A.st_blocks, R.u, R.total);
+        UnitDesc nxt = unit_desc(un, wn);
         prestaged = false;
-        /* the staged text is dead unless this unit's write needs it: bring in the next unit's text under the assembly and the writes */
-        if (!R.needs_text && nxt.valid && nxt.db > nxt.da) { H.stage(S, (const void *)(uintptr_t)nxt.base_abs, desc_load(nxt)); prestaged = true; }
+        /* the staged text is dead unless this unit's write needs it: bring in the next unit's text, and its document offsets, under the
+         * assembly and the writes */
+        if (!R.needs_text && nxt.valid && nxt.db > nxt.da) {
+            H.stage(S, (const void *)(uintptr_t)nxt.base_abs, desc_load(nxt));
+            if (lane <= nxt.db - nxt.da) nxt.doff = A.doc_off[nxt.da + lane];
+            prestaged = true;
+        }
         OBMW_PC_MARK(PC_OTHER);
         if (have_pend) {
             const uint64_t base = chain_resolve(A.st_tuples, A.st_blocks, pend.u, nblocks);

@@ -351,6 +351,25 @@ OBM_HD void wrec_unit(const WRec &r, uint32_t k, uint32_t &da, uint32_t &db, uin
     else { db = da + DMAX < group_end ? da + DMAX : group_end; if (da > db) da = db; }
     extra = (large && k == r.n_units - 1) ? 1u : 0u;
 }
+/* ---- unit descriptor (16 bytes, one load when a warp takes the unit), written by k_wunit_descs / the host replay:
+ * documents [da, da + nd), extra, the text's span doc_off[da + nd] - doc_off[da] (at most BUFB: a unit fits the buffer)
+ * and its byte offset doc_off[da] ---- */
+struct alignas(16) WUnit { uint32_t da; uint32_t nd_span; /* nd 0..5 | extra 7 | span 8.. */ uint64_t off; };
+OBM_HD WUnit pack_wunit(const uint64_t *doc_off, uint32_t da, uint32_t db, uint32_t extra) {
+    const uint64_t off = doc_off[da];
+    const uint32_t span = db > da ? (uint32_t)(doc_off[db] - off) : 0u;
+    return WUnit{da, (db - da) | (extra << 7) | (span << 8), off};
+}
+/* unit k of tile record r */
+OBM_HD WUnit make_wunit(const uint64_t *doc_off, const WRec &r, uint32_t k) {
+    uint32_t da, db, extra;
+    wrec_unit(r, k, da, db, extra);
+    return pack_wunit(doc_off, da, db, extra);
+}
+OBM_HD uint32_t wu_nd(const WUnit &w) { return w.nd_span & 0x3Fu; }
+OBM_HD uint32_t wu_extra(const WUnit &w) { return (w.nd_span >> 7) & 1u; }
+OBM_HD uint32_t wu_span(const WUnit &w) { return w.nd_span >> 8; }
+static_assert(DMAX < 64 && BUFB < (1u << 24), "the descriptor packs nd in 6 bits and the span in 24");
 
 } /* namespace obmw */
 #endif

@@ -77,30 +77,36 @@ static_assert(STEP == 64 * 32 && STEP == 2 * ROW && (BUFB + STEP - 1) / STEP * 2
 struct UnitRegs {
     uint32_t u, da, nd, extra, n_owners, n_ml, n_small /* tuples of the unit's small documents */; uint64_t total; bool needs_text;
     bool paged; /* more owning lines than OWN_CAP: the unit is scanned (and later written) one document at a time */
+    bool long_line; /* an owner's line number exceeds the packed tuple's (ST_MAXLEN): the unit cannot take the deferred write */
     uint32_t dflag, dtot, dexcl, dlen; /* lane d < nd: document da + d */
 };
 
 struct WArgs {
     const uint8_t *bytes; const uint64_t *doc_off; uint32_t ndocs; uint64_t total_bytes;
     const uint32_t *tile_first; uint32_t ntiles;
-    const WRec *wrec; const uint64_t *ubase; /* [ntiles + 1] exclusive scan of units per tile */
-    const uint32_t *unit_tile;               /* [units] tile of every unit (device: units are handed out one by one) */
+    const uint64_t *ubase;                   /* [ntiles + 1] exclusive scan of units per tile */
+    const WUnit *units;                      /* [units] descriptor of every unit (device: units are handed out one by one) */
     uint64_t *st_tuples, *st_blocks;         /* chain over the units' tuple counts (obm_warp.cuh: chain_publish / chain_resolve) */
     uint64_t units_max;                      /* capacity the chain arrays were carved for */
     const uint32_t *counts;                  /* tuple counts of large documents (k_large_resolve) */
     obm_tuple *out; uint64_t out_cap; uint64_t *tuple_off;
     uint32_t *status; unsigned long long *totals; uint32_t *ctl;
 };
-/* where a unit's text lies: computed ahead of the unit so that its bulk copy can be issued early */
-struct UnitDesc { uint32_t u, da, db, extra, skew, span; uint64_t base_abs; bool valid; };
-OBM_HD UnitDesc make_desc(const WArgs &A, uint32_t u, uint32_t da, uint32_t db, uint32_t extra) {
-    UnitDesc d{u, da, db, extra, 0, 0, 0, true};
-    if (db > da) {
-        const uint64_t b0 = A.doc_off[da], b1 = A.doc_off[db];
-        const uint64_t abs0 = (uint64_t)(uintptr_t)A.bytes + b0;
-        d.base_abs = abs0 & ~15ull; d.skew = (uint32_t)(abs0 - d.base_abs); d.span = (uint32_t)(b1 - b0) + d.skew;
+/* where a unit's text lies: computed ahead of the unit so that its bulk copy can be issued early.  doff: doc_off[da + lane]
+ * on lanes 0..nd once the caller has loaded it with the prestaged copy (compute_unit loads it otherwise) */
+struct UnitDesc { uint32_t u, da, db, extra, skew, span; uint64_t base_abs; bool valid; uint64_t doff; };
+OBM_HD UnitDesc make_desc(const WArgs &A, uint32_t u, const WUnit &w) {
+    const uint32_t nd = wu_nd(w);
+    UnitDesc d{u, w.da, w.da + nd, wu_extra(w), 0, 0, 0, true, 0};
+    if (nd) {
+        const uint64_t abs0 = (uint64_t)(uintptr_t)A.bytes + w.off;
+        d.base_abs = abs0 & ~15ull; d.skew = (uint32_t)(abs0 - d.base_abs); d.span = wu_span(w) + d.skew;
     }
     return d;
+}
+/* documents [da, db) of the batch as a unit: the same descriptor the set-up kernels write */
+OBM_HD UnitDesc make_desc(const WArgs &A, uint32_t u, uint32_t da, uint32_t db, uint32_t extra) {
+    return make_desc(A, u, pack_wunit(A.doc_off, da, db, extra));
 }
 OBM_HD uint32_t desc_load(const UnitDesc &d) { return (d.span + 15u) & ~15u; }
 
@@ -205,7 +211,7 @@ OBMW_DEV bool scan_range(WarpSmem &W, UnitSet &S, const WArgs &A, const obm::Tab
     (void)A;
     const uint32_t lane = WLANE();
     uint32_t n_owners = 0, n_ml = 0;
-    bool unstaged = false;
+    bool unstaged = false, long_line = false;
     if (nd) {
         const auto text = WTEXT(W);
 
@@ -341,6 +347,7 @@ OBMW_DEV bool scan_range(WarpSmem &W, UnitSet &S, const WArgs &A, const obm::Tab
                 if (df & DF_EXACT) { S.orec[o] = make_orec(ls - dpos, first - dpos, 0, false, false, true, d, 0); S.opos[o] = 0; }
                 else {
                     const uint32_t line = 1 + w_nl_before(W, S, ls) - w_nl_before(W, S, dpos);
+                    long_line |= line > ST_MAXLEN;
                     const uint32_t c = text[first];
                     uint32_t plus = first;
                     marker = c == '+';
@@ -453,11 +460,13 @@ OBMW_DEV bool scan_range(WarpSmem &W, UnitSet &S, const WArgs &A, const obm::Tab
     R.dflag = dflag; R.dtot = dtot; R.dexcl = dexcl; R.dlen = dlen;
     R.needs_text = WBALLOT(unstaged || dflag != 0) != 0;
     R.paged = false;
+    R.long_line = WBALLOT(long_line) != 0;
     OBMW_PC_MARK(PC_ASM);
     return true;
 }
 
-/* ---- first half of a unit: stage its text, scan it, assemble the tuple positions ---- */
+/* ---- first half of a unit: stage its text, scan it, assemble the tuple positions.  prestaged: the caller has issued the
+ * text's bulk copy and, with it, loaded D.doff ---- */
 template <class Hooks>
 OBMW_DEV void compute_unit(WarpSmem &W, UnitSet &S, const WArgs &A, const obm::Tables &T, Hooks &H, const UnitDesc &D, bool prestaged, UnitRegs &R OBMW_PC_PARAM) {
     const uint32_t lane = WLANE();
@@ -467,8 +476,9 @@ OBMW_DEV void compute_unit(WarpSmem &W, UnitSet &S, const WArgs &A, const obm::T
         const uint32_t skew = D.skew, span = D.span, load = desc_load(D);
         const uint64_t b0 = (D.base_abs + skew) - (uint64_t)(uintptr_t)A.bytes;
         lo_pos = skew; hi_pos = span;
-        if (!prestaged) H.stage(W, (const void *)(uintptr_t)D.base_abs, load);
-        if (lane <= nd) W.dstart[lane] = (uint32_t)(A.doc_off[da + lane] - b0) + skew;
+        uint64_t doff = D.doff;
+        if (!prestaged) { H.stage(W, (const void *)(uintptr_t)D.base_abs, load); if (lane <= nd) doff = A.doc_off[da + lane]; }
+        if (lane <= nd) W.dstart[lane] = (uint32_t)(doff - b0) + skew;
         if (lane < nd) W.dflag[lane] = 0;
         WSYNC();
         H.stage_wait(W, load);
@@ -514,18 +524,24 @@ OBMW_DEV void compute_unit(WarpSmem &W, UnitSet &S, const WArgs &A, const obm::T
     if (extra) R.total += A.counts[da + nd];
 }
 
+/* staged marker tuples: staged line k (lane k < ns) holds c tuples whose place is [rel, rel + c) inside the unit;
+ * put(position, packed tuple) stores one.  A line per round, a lane per tuple */
+template <class Put>
+OBMW_DEV void copy_staged(const UnitSet &S, uint32_t ns, uint32_t c, uint32_t rel, Put put) {
+    const uint32_t lane = WLANE();
+    for (uint32_t k = 0; k < ns; k++) {
+        const uint32_t ck = WSHFL(c, k), rk = WSHFL(rel, k);
+        if (lane < ck) put(rk + lane, S.u.c.stage[k * LTS + lane]);
+    }
+}
+
 /* ---- deferred path: the unit's tuples packed into W.fin in final order (only units without needs_text) -------
  * Returns false when the unit does not fit (more than FIN_CAP tuples, a line number beyond the packed form): the
  * caller then writes it directly (write_unit). */
 OBMW_DEV bool assemble_fin(WarpSmem &W, UnitSet &S, const UnitRegs &R, WAcc &acc) {
     const uint32_t lane = WLANE();
     const uint32_t nd = R.nd, n_owners = R.n_owners, n_ml = R.n_ml;
-    bool bad = R.n_small > FIN_CAP;
-    for (uint32_t o0 = 0; o0 < n_owners && !bad; o0 += 32) {
-        const uint32_t o = o0 + lane;
-        if (o < n_owners && or_line(S.orec[o]) > ST_MAXLEN) bad = true;
-    }
-    if (WBALLOT(bad)) return false;
+    if (R.n_small > FIN_CAP || R.long_line) return false;
     if (lane < nd) { W.fin[R.dexcl + R.dtot - 1u] = st_pack(OBM_K_EOF, R.dlen, 0); acc.lexemes++; }
     for (uint32_t o0 = 0; o0 < n_owners; o0 += 32) {
         const uint32_t o = o0 + lane;
@@ -544,10 +560,7 @@ OBMW_DEV bool assemble_fin(WarpSmem &W, UnitSet &S, const UnitRegs &R, WAcc &acc
             const uint32_t ms = S.u.c.mstat[lane]; /* never MS_NONE here: every marker line with tuples is staged */
             if (ms != MS_NONE) { c = ms >> 16; rel = S.opos[S.mlist[lane]]; acc.markers += ms & 0xFFu; acc.lexemes += (ms >> 8) & 0xFFu; }
         }
-        for (uint32_t k = 0; k < ns; k++) {
-            const uint32_t ck = WSHFL(c, k), rk = WSHFL(rel, k);
-            if (lane < ck) W.fin[rk + lane] = S.u.c.stage[k * LTS + lane];
-        }
+        copy_staged(S, ns, c, rel, [&](uint32_t at, uint32_t v) { W.fin[at] = v; });
     }
     WSYNC();
     return true;
@@ -660,7 +673,7 @@ OBMW_DEV void write_range(WarpSmem &W, UnitSet &S, const WArgs &A, const obm::Ta
             }
         }
     }
-    /* staged marker tuples: line after line, a lane per tuple (a line's tuples are contiguous on both sides) */
+    /* staged marker tuples (a line's tuples are contiguous on both sides) */
     {
         const uint32_t ns = n_ml < MLCAP ? n_ml : MLCAP;
         uint32_t c = 0, rel = 0;
@@ -672,13 +685,7 @@ OBMW_DEV void write_range(WarpSmem &W, UnitSet &S, const WArgs &A, const obm::Ta
                 acc.markers += ms & 0xFFu; acc.lexemes += (ms >> 8) & 0xFFu;
             }
         }
-        if (writing) {
-            for (uint32_t k = 0; k < ns; k++) {
-                const uint32_t ck = WSHFL(c, k), rk = WSHFL(rel, k);
-                const uint64_t at = base + rk + lane;
-                if (lane < ck && at < A.out_cap) A.out[at] = st_unpack(S.u.c.stage[k * LTS + lane]);
-            }
-        }
+        if (writing) copy_staged(S, ns, c, rel, [&](uint32_t f, uint32_t v) { if (base + f < A.out_cap) A.out[base + f] = st_unpack(v); });
     }
     WSYNC();
 }
