@@ -186,7 +186,7 @@ k_warp_scan(WArgs A) {
         prestaged = false;
         /* the staged text is dead unless this unit's write needs it: bring in the next unit's text, and its document offsets, under the
          * assembly and the writes */
-        if (!R.needs_text && nxt.valid && nxt.db > nxt.da) {
+        if (prestage_next(R, nxt)) {
             H.stage(S, (const void *)(uintptr_t)nxt.base_abs, desc_load(nxt));
             if (lane <= nxt.db - nxt.da) nxt.doff = A.doc_off[nxt.da + lane];
             prestaged = true;

@@ -109,6 +109,10 @@ OBM_HD UnitDesc make_desc(const WArgs &A, uint32_t u, uint32_t da, uint32_t db, 
     return make_desc(A, u, pack_wunit(A.doc_off, da, db, extra));
 }
 OBM_HD uint32_t desc_load(const UnitDesc &d) { return (d.span + 15u) & ~15u; }
+/* may the warp stage unit nxt's text (and load its document offsets) as soon as unit R is scanned?  Only when R's write
+ * never reads the staged text again: R takes the deferred write, or the direct write of a unit without needs_text
+ * (more than FIN_CAP tuples, long_line), which writes from the owner records and the staged marker tuples alone */
+OBM_HD bool prestage_next(const UnitRegs &R, const UnitDesc &nxt) { return !R.needs_text && nxt.valid && nxt.db > nxt.da; }
 
 struct WAcc { uint32_t markers, lexemes, exact, fatal; };
 constexpr uint32_t MS_NONE = 0xFFFFFFFFu;

@@ -46,6 +46,12 @@ def lib():
         L.hs_pipe_batch.argtypes = L.hs_tile_batch.argtypes
         L.hs_warp_batch.restype = ctypes.c_uint64
         L.hs_warp_batch.argtypes = L.hs_tile_batch.argtypes
+        L.hs_warp_batch_report.restype = ctypes.c_uint64
+        L.hs_warp_batch_report.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_uint32, ctypes.c_void_p, ctypes.c_uint64,
+                                           ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_uint64,
+                                           ctypes.POINTER(ctypes.c_uint64)]
+        L.hs_warp_units.restype = ctypes.c_uint64
+        L.hs_warp_units.argtypes = [ctypes.c_void_p, ctypes.c_uint32]
         L.hs_large_doc.restype = ctypes.c_uint64
         L.hs_large_doc.argtypes = [ctypes.c_char_p, ctypes.c_uint32, ctypes.c_void_p, ctypes.c_uint64, ctypes.POINTER(ctypes.c_uint32)]
         L.hs_large_chunk_starts.restype = ctypes.c_uint32
@@ -116,25 +122,64 @@ def fmt_tuples(tuples):
     return [(names.get(int(t) >> 59, int(t) >> 59), int(t) & 0xFFFFFFFF, (int(t) >> 32) & 0x7FFFFFF) for t in tuples]
 
 
+BAD_STARTS = (1 << 64) - 1  # hs_warp_batch*: a unit's document starts differed from doc_off
+
+
+def _place(docs, skew):
+    """the batch at address 16k + skew inside a poisoned buffer (readable around it, like the device buffer contract)
+    -> (buffer, batch view, doc_off, output capacity)"""
+    payload = b"".join(docs)
+    buf = np.full(len(payload) + 96, 0x2B, dtype=np.uint8)
+    start = (-buf.ctypes.data) % 16 + 16 + (skew & 15)
+    buf[start:start + len(payload)] = np.frombuffer(payload, dtype=np.uint8)
+    off = np.zeros(len(docs) + 1, dtype=np.uint64)
+    if docs:
+        off[1:] = np.cumsum([len(d) for d in docs])
+    return buf, buf[start:], off, 2 * int(off[-1]) + 2 * len(docs) + 16
+
+
 def tile_batch(docs, skew=0, pipeline=False):
     """Emulation of the device fast paths (pipeline=0 r01 fused tile kernel, 1 r01 two-stage pipeline, 2 the fused warp
     kernel of mode 0, run by 32 fibers per warp) over a list of documents
     -> (tuples, doc_tuple_off, stats)."""
     L = lib()
-    # the batch sits at address = 16k + skew inside a poisoned buffer (readable around it, like the device buffer contract)
-    payload = b"".join(docs)
-    buf = np.full(len(payload) + 96, 0x2B, dtype=np.uint8)
-    start = (-buf.ctypes.data) % 16 + 16 + (skew & 15)
-    buf[start:start + len(payload)] = np.frombuffer(payload, dtype=np.uint8)
-    data = buf[start:]
-    off = np.zeros(len(docs) + 1, dtype=np.uint64)
-    if docs:
-        off[1:] = np.cumsum([len(d) for d in docs])
-    cap = 2 * int(off[-1]) + 2 * len(docs) + 16
+    _buf, data, off, cap = _place(docs, skew)
     out = np.zeros(cap, dtype=np.uint64)
     toff = np.zeros(len(docs) + 1, dtype=np.uint64)
     stats = np.zeros(4, dtype=np.uint64)
     fn = {0: L.hs_tile_batch, 1: L.hs_pipe_batch, 2: L.hs_warp_batch}[int(pipeline)]
     n = fn(data.ctypes.data, off.ctypes.data, len(docs), out.ctypes.data, cap, toff.ctypes.data, skew, stats.ctypes.data)
+    assert n != BAD_STARTS, "the warp replay's document starts differ from doc_off"
     assert n <= cap
     return out[:n].copy(), toff, stats
+
+
+# one row per unit of warp_batch's report
+WARP_REPORT = np.dtype([(f, np.uint32) for f in ("u", "da", "nd", "extra", "needs_text", "paged", "deferred", "over_fin",
+                                                  "long_line", "prestaged")])
+
+
+def warp_batch(docs, skew=0):
+    """The fused warp kernel's software pipeline replayed in k_warp_scan's order (hs_warp_batch_report), with the next
+    unit's text staged over the dead text as early as the kernel stages it -> (tuples, doc_tuple_off, stats, report):
+    report[u] says how unit u went (nd, extra, needs_text, paged, deferred write, more than FIN_CAP tuples, long_line,
+    and whether its text was prestaged)"""
+    L = lib()
+    _buf, data, off, cap = _place(docs, skew)
+    out = np.zeros(cap, dtype=np.uint64)
+    toff = np.zeros(len(docs) + 1, dtype=np.uint64)
+    stats = np.zeros(4, dtype=np.uint64)
+    rcap = warp_units(off)
+    report = np.zeros(rcap, dtype=WARP_REPORT)
+    nu = ctypes.c_uint64()
+    n = L.hs_warp_batch_report(data.ctypes.data, off.ctypes.data, len(docs), out.ctypes.data, cap, toff.ctypes.data,
+                               stats.ctypes.data, report.ctypes.data, rcap, ctypes.byref(nu))
+    assert n != BAD_STARTS, "the warp replay's document starts differ from doc_off"
+    assert n <= cap and nu.value == rcap
+    return out[:n].copy(), toff, stats, report
+
+
+def warp_units(doc_off):
+    """number of units the fused warp kernel cuts the batch into (make_wrec over its tiles)"""
+    off = np.ascontiguousarray(doc_off, dtype=np.uint64)
+    return int(lib().hs_warp_units(off.ctypes.data, len(off) - 1))

@@ -511,20 +511,48 @@ static uint64_t g_wstat_fast = 0, g_wstat_generic = 0;
 #include "../../operator-builder_b200/csrc/obm_warp_core.h"
 extern "C" void hs_warp_line_stats(uint64_t *fast, uint64_t *generic) { *fast = g_wstat_fast; *generic = g_wstat_generic; }
 
+
 namespace {
+/* bytes that a read of dead text would turn into tuples: line starts, markers, comments, scopes, values, an unterminated
+ * back-tick string, and bytes >= 0x80 (the exact lexer) -- in a phase that shifts from one staging to the next */
+const uint8_t POISON[] = {'\n', '+', '#', '/', ':', '=', '`', 0x80, 0xff};
 struct HostHooks {
-    void stage(obmw::WarpSmem &S, const void *gsrc, uint32_t nbytes) {
-        if (wemu::lane() == 0) memcpy(S.text, gsrc, nbytes); /* whatever the previous unit left behind stays in the buffer, like on the device */
+    const uint64_t *doc_off = nullptr;
+    uint32_t da = 0, nd = 0, skew = 0; /* the unit being scanned: what compute_unit must have put in W.dstart */
+    uint32_t shift = 0;
+    uint64_t bad_starts = 0;
+    void poison(obmw::WarpSmem &S) {
+        for (size_t i = 0; i < sizeof S.text; i++) S.text[i] = POISON[(i + shift) % sizeof POISON];
+        shift++;
     }
-    void stage_wait(obmw::WarpSmem &, uint32_t) {}
+    /* the device's bulk copy, landed at once over text that is dead by the pipeline's rules */
+    void stage(obmw::WarpSmem &S, const void *gsrc, uint32_t nbytes) {
+        if (wemu::lane() == 0) { poison(S); memcpy(S.text, gsrc, nbytes); }
+    }
+    /* compute_unit has written the document starts (from D.doff when prestaged): check them against doc_off, and put the
+     * right ones in place so that a wrong start is reported instead of sending the scan outside the buffer */
+    void stage_wait(obmw::WarpSmem &S, uint32_t) {
+        const uint32_t l = wemu::lane();
+        if (l > nd) return;
+        const uint32_t want = (uint32_t)(doc_off[da + l] - doc_off[da]) + skew;
+        if (S.dstart[l] != want) {
+            if (bad_starts++ < 4) fprintf(stderr, "hostsim: documents [%u, %u]: dstart[%u] = %u, doc_off gives %u\n", da, da + nd, l, S.dstart[l], want);
+            S.dstart[l] = want;
+        }
+    }
 };
 }
 
-/* the same software pipeline as k_warp_scan (one warp processes every unit in order): scan unit i, "publish", write unit
- * i - 1 from its UnitSet while the text buffer already holds unit i, ... */
-extern "C" uint64_t hs_warp_batch(const uint8_t *bytes, const uint64_t *doc_off, uint32_t ndocs, obm_tuple *out, uint64_t cap,
-                                  uint64_t *tuple_off, uint32_t fake_skew, uint64_t *stats) {
-    (void)fake_skew;
+/* one row of hs_warp_batch_report per unit, in unit order */
+enum { WREP_U, WREP_DA, WREP_ND, WREP_EXTRA, WREP_NEEDS_TEXT, WREP_PAGED, WREP_DEFERRED, WREP_OVER_FIN, WREP_LONG_LINE, WREP_PRESTAGED, WREP_N };
+
+/* The software pipeline of k_warp_scan, in its order, by one warp that takes every unit in id order (which is what the
+ * look-back chain enforces): scan unit i, publish its count, take unit i + 1's descriptor and -- where prestage_next allows
+ * it -- stage its text at once over unit i's and load its document offsets lane by lane, then write unit i - 1 from
+ * W.fin, then assemble unit i into W.fin or write it directly.  Large documents are counted before the loop (the side
+ * stream) and filled after it.  Returns the tuple count, or ~0 when a unit's document starts were wrong. */
+extern "C" uint64_t hs_warp_batch_report(const uint8_t *bytes, const uint64_t *doc_off, uint32_t ndocs, obm_tuple *out, uint64_t cap,
+                                         uint64_t *tuple_off, uint64_t *stats, uint32_t *report, uint64_t report_cap, uint64_t *n_units) {
     using namespace obmw;
     static WarpSmem S; static wemu::Warp W; static bool poisoned = false;
     if (!poisoned) { memset(&S, 0x2B, sizeof S); poisoned = true; }
@@ -535,6 +563,7 @@ extern "C" uint64_t hs_warp_batch(const uint8_t *bytes, const uint64_t *doc_off,
     WArgs A; memset(&A, 0, sizeof A);
     A.bytes = bytes; A.doc_off = doc_off; A.ndocs = ndocs; A.total_bytes = total; A.ntiles = (uint32_t)ntiles;
     A.counts = counts.data(); A.out = out; A.out_cap = cap; A.tuple_off = tuple_off; A.status = status; A.totals = totals;
+    /* k_wtile_index, k_wunits, the scan, k_wunit_descs */
     std::vector<WRec> recs(ntiles); std::vector<uint64_t> ubase(ntiles + 1, 0);
     uint32_t d = 0;
     for (uint64_t t = 0; t < ntiles; t++) {
@@ -544,37 +573,66 @@ extern "C" uint64_t hs_warp_batch(const uint8_t *bytes, const uint64_t *doc_off,
         ubase[t + 1] = ubase[t] + recs[t].n_units;
     }
     const uint32_t nunits = (uint32_t)ubase[ntiles];
-    HostHooks H;
+    std::vector<WUnit> units(nunits);
+    for (uint64_t t = 0; t < ntiles; t++)
+        for (uint32_t k = 0; k < recs[t].n_units; k++) units[ubase[t] + k] = make_wunit(doc_off, recs[t], k);
+    A.ubase = ubase.data(); A.units = units.data();
+    if (n_units) *n_units = nunits;
     uint64_t st_m = 0, st_l = 0, st_e = 0, st_f = 0, chain = 0;
-    UnitRegs pend[32]; uint64_t pend_base = 0; bool have_pend = false;
+    /* k_large_count: every large document before the scan */
     std::vector<uint32_t> large_docs;
+    for (const WUnit &w : units) {
+        if (!wu_extra(w)) continue;
+        const uint32_t dl = w.da + wu_nd(w);
+        obm::SmallSink s(nullptr, 0); obm::Lexer<obm::SmallSink> lx(TBL, bytes + doc_off[dl], (uint32_t)(doc_off[dl + 1] - doc_off[dl]), s);
+        const int st = lx.run<false>(); counts[dl] = s.n_tuples; st_m += s.n_markers; st_l += s.n_lexemes; st_e++; st_f += st == obm::RUN_FATAL;
+        large_docs.push_back(dl);
+    }
+    HostHooks H; H.doc_off = doc_off;
     auto add_acc = [&](WAcc *a) { for (int l = 0; l < 32; l++) { st_m += a[l].markers; st_l += a[l].lexemes; st_e += a[l].exact; st_f += a[l].fatal; } };
-    for (uint64_t t = 0; t < ntiles; t++) {
-        for (uint32_t k = 0; k < recs[t].n_units; k++) {
-            uint32_t da, db, extra;
-            wrec_unit(recs[t], k, da, db, extra);
-            if (extra) { /* the large path (k_large_*): counted before the scan, filled after it */
-                const uint32_t dl = db;
-                obm::SmallSink s(nullptr, 0); obm::Lexer<obm::SmallSink> lx(TBL, bytes + doc_off[dl], (uint32_t)(doc_off[dl + 1] - doc_off[dl]), s);
-                int st = lx.run<false>(); counts[dl] = s.n_tuples; st_m += s.n_markers; st_l += s.n_lexemes; st_e++; st_f += st == obm::RUN_FATAL;
-                large_docs.push_back(dl);
-            }
-            const uint32_t u = (uint32_t)ubase[t] + k;
-            UnitRegs R[32];
-            const UnitDesc D = make_desc(A, u, da, db, extra);
-            wemu::run(W, [&]() { compute_unit(S, S.set, A, TBL, H, D, false, R[wemu::lane()]); });
-            const uint64_t my_base = chain; chain += R[0].total; /* publish */
-            if (have_pend) { wemu::run(W, [&]() { write_fin(S, A, pend[wemu::lane()], nunits, pend_base); }); have_pend = false; }
-            WAcc a[32]; memset(a, 0, sizeof a);
-            bool deferred[32]; memset(deferred, 0, sizeof deferred);
-            if (!R[0].needs_text) wemu::run(W, [&]() { deferred[wemu::lane()] = assemble_fin(S, S.set, R[wemu::lane()], a[wemu::lane()]); });
-            if (deferred[0]) { memcpy(pend, R, sizeof R); pend_base = my_base; have_pend = true; }
-            else wemu::run(W, [&]() { write_unit(S, S.set, A, TBL, R[wemu::lane()], nunits, my_base, a[wemu::lane()]); });
-            add_acc(a);
+    /* the descriptor of unit u as every lane holds it (doff: not loaded) */
+    auto unit_desc = [&](uint32_t u, UnitDesc *D) {
+        for (int l = 0; l < 32; l++) {
+            if (u < nunits) D[l] = make_desc(A, u, units[u]);
+            else { D[l] = UnitDesc{0, 0, 0, 0, 0, 0, 0, false, 0}; }
         }
+    };
+    UnitRegs pend[32]; bool have_pend = false;
+    uint64_t pend_base = 0;
+    UnitDesc cur[32], nxt[32];
+    unit_desc(0, cur);
+    bool prestaged = false;
+    while (cur[0].valid) {
+        UnitRegs R[32];
+        H.da = cur[0].da; H.nd = cur[0].db - cur[0].da; H.skew = cur[0].skew;
+        wemu::run(W, [&]() { compute_unit(S, S.set, A, TBL, H, cur[wemu::lane()], prestaged, R[wemu::lane()]); });
+        const uint64_t my_base = chain; chain += R[0].total; /* publish */
+        unit_desc(cur[0].u + 1, nxt);
+        const bool pre = prestage_next(R[0], nxt[0]);
+        if (pre) { /* the next unit's bulk copy, as if it landed at once, and its document offsets, a lane each */
+            H.poison(S);
+            memcpy(S.text, (const void *)(uintptr_t)nxt[0].base_abs, desc_load(nxt[0]));
+            for (uint32_t l = 0; l <= nxt[0].db - nxt[0].da; l++) nxt[l].doff = doc_off[nxt[0].da + l];
+        }
+        if (have_pend) { wemu::run(W, [&]() { write_fin(S, A, pend[wemu::lane()], nunits, pend_base); }); have_pend = false; }
+        WAcc a[32]; memset(a, 0, sizeof a);
+        bool deferred[32]; memset(deferred, 0, sizeof deferred);
+        if (!R[0].needs_text) wemu::run(W, [&]() { deferred[wemu::lane()] = assemble_fin(S, S.set, R[wemu::lane()], a[wemu::lane()]); });
+        if (deferred[0]) { memcpy(pend, R, sizeof R); pend_base = my_base; have_pend = true; }
+        else wemu::run(W, [&]() { write_unit(S, S.set, A, TBL, R[wemu::lane()], nunits, my_base, a[wemu::lane()]); });
+        add_acc(a);
+        const uint32_t u = cur[0].u;
+        if (report && u < report_cap) {
+            uint32_t *r = report + (uint64_t)u * WREP_N;
+            r[WREP_U] = u; r[WREP_DA] = cur[0].da; r[WREP_ND] = R[0].nd; r[WREP_EXTRA] = R[0].extra;
+            r[WREP_NEEDS_TEXT] = R[0].needs_text; r[WREP_PAGED] = R[0].paged; r[WREP_DEFERRED] = deferred[0];
+            r[WREP_OVER_FIN] = R[0].n_small > FIN_CAP; r[WREP_LONG_LINE] = R[0].long_line; r[WREP_PRESTAGED] = prestaged;
+        }
+        memcpy(cur, nxt, sizeof cur);
+        prestaged = pre;
     }
     if (have_pend) wemu::run(W, [&]() { write_fin(S, A, pend[wemu::lane()], nunits, pend_base); });
-    for (uint32_t dl : large_docs) {
+    for (uint32_t dl : large_docs) { /* k_large_fill */
         const uint64_t at = tuple_off[dl];
         obm::WriteSink sink(out + at, at < cap ? cap - at : 0);
         obm::Lexer<obm::WriteSink> lx(TBL, bytes + doc_off[dl], (uint32_t)(doc_off[dl + 1] - doc_off[dl]), sink);
@@ -582,5 +640,22 @@ extern "C" uint64_t hs_warp_batch(const uint8_t *bytes, const uint64_t *doc_off,
     }
     if (ndocs == 0) tuple_off[0] = 0;
     if (stats) { stats[0] = st_m; stats[1] = st_l; stats[2] = st_e; stats[3] = st_f; }
-    return chain;
+    return H.bad_starts ? ~0ull : chain;
+}
+extern "C" uint64_t hs_warp_batch(const uint8_t *bytes, const uint64_t *doc_off, uint32_t ndocs, obm_tuple *out, uint64_t cap,
+                                  uint64_t *tuple_off, uint32_t fake_skew, uint64_t *stats) {
+    (void)fake_skew; /* the skew is the batch's address (tests/hostsim/__init__.py) */
+    return hs_warp_batch_report(bytes, doc_off, ndocs, out, cap, tuple_off, stats, nullptr, 0, nullptr);
+}
+/* units of the batch (k_wunits + the scan): what k_warp_scan's warps share */
+extern "C" uint64_t hs_warp_units(const uint64_t *doc_off, uint32_t ndocs) {
+    const uint64_t ntiles = doc_off[ndocs] / obmw::TILE + 1;
+    uint64_t n = 0;
+    uint32_t d = 0;
+    for (uint64_t t = 0; t < ntiles; t++) {
+        const uint32_t d0 = d;
+        while (d < ndocs && doc_off[d] < (t + 1) * (uint64_t)obmw::TILE) d++;
+        n += obmw::make_wrec(doc_off, d0, d).n_units;
+    }
+    return n;
 }

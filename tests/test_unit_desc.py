@@ -96,8 +96,9 @@ def test_descriptor_table_matches_the_tile_records(unit_desc_lib, name, skew):
 @pytest.mark.parametrize("name", sorted(batches()) + ["dense"])
 @pytest.mark.parametrize("skew", [0, 3, 13])
 def test_mode0_stream_equals_the_exact_path(name, skew):
-    """k_warp_scan reads the descriptors, prestages the next unit's document offsets and resolves the chain in one round:
-    tuple for tuple what the exact path (mode 1) writes, also at bases that are not 16-byte aligned"""
+    """k_warp_scan reads the descriptors and resolves the chain in one round: tuple for tuple what the exact path (mode 1)
+    writes, also at bases that are not 16-byte aligned.  These batches are too small for a warp to get a second unit, so
+    the staging of a unit's text and offsets under its predecessor's writes is not exercised here (test_warp_pipeline.py)"""
     import torch
     import operator_builder_b200 as ob
     docs = [dense_doc(4096, i) for i in range(300)] + [doc_of(4096, 1)] * 20 + [dense_doc(4096, 7)] * 100 if name == "dense" else batches()[name]
