@@ -9,7 +9,7 @@
  *   error.go:18,40   "%s at position: %+v, following %q"
  *   state.go:193     "unmatched string delimiter %s at position %+v, following %q"
  *   state.go:259,270 "invalid float|integer literal %q: %s before position %d"
- * `%q` is strconv.Quote, `%+v`/`%d` of position{line,column} print {line:L column:C} / {L C}.
+ * `%q` is strconv.Quote (obm_quote.h), `%+v`/`%d` of position{line,column} print {line:L column:C} / {L C}.
  */
 #include <cstdint>
 #include <cstdio>
@@ -20,6 +20,7 @@
 #include "../../include/obmarkers.h"
 #include "go_unicode_tables.h"
 #include "obm_core.h"
+#include "obm_quote.h"
 
 namespace {
 
@@ -29,8 +30,6 @@ const obm::Tables &host_tables() {
     static const obm::Tables T = { GO_LETTER_RANGES, GO_LETTER_RANGES_N, GO_NUMBER_RANGES, GO_NUMBER_RANGES_N, F64_OVERFLOW_DIGITS };
     return T;
 }
-
-bool is_print(int r) { return r >= 0 && obm::in_ranges(GO_PRINT_RANGES, GO_PRINT_RANGES_N, r); }
 
 /* Each invalid byte of input becomes U+FFFD in a Value: next() does `buffer += string(r)` with
  * r == utf8.RuneError (position.go:21,36). */
@@ -46,37 +45,6 @@ void append_sanitized(std::string &dst, const uint8_t *p, uint64_t n) {
         } else i += w;
     }
     dst.append((const char *)p + run, n - run);
-}
-
-/* strconv.Quote */
-void go_quote(std::string &out, const std::string &s) {
-    static const char hex[] = "0123456789abcdef";
-    const uint8_t *b = (const uint8_t *)s.data();
-    uint32_t n = (uint32_t)s.size();
-    out.push_back('"');
-    uint32_t i = 0;
-    while (i < n) {
-        uint32_t w = 1; int r = b[i];
-        if (r >= 0x80) r = obm::decode_rune(b, i, n, w);
-        if (w == 1 && r == obm::RUNE_ERR) { out += "\\x"; out.push_back(hex[b[i] >> 4]); out.push_back(hex[b[i] & 0xF]); i += 1; continue; }
-        if (r == '"' || r == '\\') { out.push_back('\\'); out.push_back((char)r); i += w; continue; }
-        if (is_print(r)) { out.append((const char *)b + i, w); i += w; continue; }
-        switch (r) {
-        case '\a': out += "\\a"; break;
-        case '\b': out += "\\b"; break;
-        case '\f': out += "\\f"; break;
-        case '\n': out += "\\n"; break;
-        case '\r': out += "\\r"; break;
-        case '\t': out += "\\t"; break;
-        case '\v': out += "\\v"; break;
-        default:
-            if (r < ' ') { out += "\\x"; out.push_back(hex[(r >> 4) & 0xF]); out.push_back(hex[r & 0xF]); }
-            else if (r < 0x10000) { out += "\\u"; for (int sh = 12; sh >= 0; sh -= 4) out.push_back(hex[(r >> sh) & 0xF]); }
-            else { out += "\\U"; for (int sh = 28; sh >= 0; sh -= 4) out.push_back(hex[(r >> sh) & 0xF]); }
-        }
-        i += w;
-    }
-    out.push_back('"');
 }
 
 struct Basis { uint64_t line; uint64_t base; uint64_t drift; };
@@ -153,7 +121,7 @@ extern "C" int obm_stream_next(obm_stream *s, obm_lexeme *out) {
             std::string v = kind == OBM_K_WARN_NOSCOPE ? "marker without scope found"
                           : kind == OBM_K_WARN_INVALID ? "invalid marker found" : "malformed argument: " + s->pending;
             v += " at position: "; put_pos(v, true, line, col);
-            v += ", following "; go_quote(v, s->last_value + s->pending);
+            v += ", following "; obm::go_quote(v, s->last_value + s->pending);
             s->cur.swap(v);
             out->type = kind == OBM_K_ERR_MALFORMED ? OBM_K_ERROR : OBM_K_WARNING;
             out->value = (const uint8_t *)s->cur.data(); out->value_len = s->cur.size(); out->line = line; out->column = col;
@@ -165,7 +133,7 @@ extern "C" int obm_stream_next(obm_stream *s, obm_lexeme *out) {
             std::string v = "unmatched string delimiter ";
             v += s->last_value.empty() ? std::string("?") : s->last_value.substr(s->last_value.size() - 1);
             v += " at position "; put_pos(v, true, s->last_line, s->last_col + 1);
-            v += ", following "; go_quote(v, s->last_value);
+            v += ", following "; obm::go_quote(v, s->last_value);
             s->cur.swap(v);
             out->type = OBM_K_ERROR; out->value = (const uint8_t *)s->cur.data(); out->value_len = s->cur.size();
             out->line = (int64_t)s->basis.line; out->column = col_of(s->basis, off);
@@ -179,9 +147,9 @@ extern "C" int obm_stream_next(obm_stream *s, obm_lexeme *out) {
                            : obm::atoi_err((const uint8_t *)lit.data(), (uint32_t)lit.size());
             int64_t line = (int64_t)s->basis.line, col = col_of(s->basis, off + len);
             std::string v = isf ? "invalid float literal " : "invalid integer literal ";
-            go_quote(v, lit);
+            obm::go_quote(v, lit);
             v += isf ? ": strconv.ParseFloat: parsing " : ": strconv.Atoi: parsing ";
-            go_quote(v, lit);
+            obm::go_quote(v, lit);
             v += code == 2 ? ": value out of range" : ": invalid syntax";
             v += " before position "; put_pos(v, false, line, col);
             s->cur.swap(v);

@@ -37,6 +37,7 @@
 #include "go_unicode_tables.h"
 #include "obm_core.h"
 #include "obm_parse_dev.h"
+#include "obm_quote.h"
 
 struct obm_registry {
     struct Def { std::string name; std::vector<std::string> args; std::vector<uint8_t> types; /* empty: untyped */ };
@@ -105,22 +106,6 @@ namespace {
 struct Lx { int32_t type; std::string value; int64_t line, col; };
 
 void put_u32(std::string &o, uint32_t v) { o.append((const char *)&v, 4); }
-
-/* strconv.Quote of the byte strings that can reach a strconv error here */
-std::string go_quote_simple(const std::string &s) {
-    static const char hex[] = "0123456789abcdef";
-    std::string o = "\"";
-    for (unsigned char c : s) {
-        if (c == '"' || c == '\\') { o.push_back('\\'); o.push_back((char)c); }
-        else if (c == '\n') o += "\\n"; else if (c == '\t') o += "\\t"; else if (c == '\r') o += "\\r";
-        else if (c == '\v') o += "\\v"; else if (c == '\f') o += "\\f";
-        else if (c < 0x20) { o += "\\x"; o.push_back(hex[c >> 4]); o.push_back(hex[c & 15]); }
-        else if (c == 0x7F) o += "\\u007f";
-        else o.push_back((char)c);
-    }
-    o.push_back('"');
-    return o;
-}
 
 bool parse_bool_ok(const std::string &v) { /* strconv.ParseBool */
     static const char *ok[] = {"1", "t", "T", "TRUE", "true", "True", "0", "f", "F", "FALSE", "false", "False"};
@@ -216,7 +201,7 @@ std::string setarg_message(uint8_t ty, uint32_t vk, const std::string &v, const 
     std::string m;
     switch (ty & obmr::TY_KIND) {
     case obmr::TY_FIELDTYPE:
-        if (vk == 3) m = "unable to unmarshal arg value " + go_quote_simple(v) + ", unable to parse field, " + v + " into FieldType";
+        if (vk == 3) m = "unable to unmarshal arg value " + obm::go_quote(v) + ", unable to parse field, " + v + " into FieldType";
         else m = "unable to unmarshal arg value, cannot convert " + go_v(vk, v) + " to string";
         break;
     default: /* string / *string / *bool: "%q" of reflect.Type (the element type for pointers) */
@@ -229,7 +214,7 @@ std::string panic_message(uint32_t vk) { return std::string("reflect.Set: value 
 std::string missing_message(const obm_registry::Def &d, uint32_t mask) {
     std::string m = "unable to inflate object, missing arguments: [";
     bool first = true;
-    for (size_t j = 0; j < d.args.size(); j++) if ((mask >> j) & 1u) { if (!first) m.push_back(' '); first = false; m += go_quote_simple(d.args[j]); }
+    for (size_t j = 0; j < d.args.size(); j++) if ((mask >> j) & 1u) { if (!first) m.push_back(' '); first = false; m += obm::go_quote(d.args[j]); }
     return m + "]";
 }
 void put_record(std::string &o, uint8_t type, const std::string &m, const std::string &text) {
@@ -347,18 +332,18 @@ struct Parser {
                 if (peeked(OBM_K_QUOTE)) next();
                 if (peeked(OBM_K_SYNTHETIC_BOOL)) {
                     std::string v = peek().value;
-                    if (!parse_bool_ok(v)) { error("strconv.ParseBool: parsing " + go_quote_simple(v) + ": invalid syntax"); st = S_STOP; break; }
+                    if (!parse_bool_ok(v)) { error("strconv.ParseBool: parsing " + obm::go_quote(v) + ": invalid syntax"); st = S_STOP; break; }
                     if (!set_argument(arg, 0, v)) { st = S_STOP; break; }
                     args.push_back(Arg{arg, 0, v}); discard();
                 } else if (consumed(OBM_K_BOOL_LITERAL)) {
-                    if (!parse_bool_ok(current.value)) { error("strconv.ParseBool: parsing " + go_quote_simple(current.value) + ": invalid syntax"); st = S_STOP; break; }
+                    if (!parse_bool_ok(current.value)) { error("strconv.ParseBool: parsing " + obm::go_quote(current.value) + ": invalid syntax"); st = S_STOP; break; }
                     if (!set_argument(arg, 0, current.value)) { st = S_STOP; break; }
                     args.push_back(Arg{arg, 0, current.value});
                 } else if (consumed(OBM_K_INTEGER_LITERAL)) {
                     if (!set_argument(arg, 1, current.value)) { st = S_STOP; break; }
                     args.push_back(Arg{arg, 1, current.value});
                 } else if (consumed(OBM_K_FLOAT_LITERAL)) {
-                    if (float32_overflows(current.value)) { error("strconv.ParseFloat: parsing " + go_quote_simple(current.value) + ": value out of range"); st = S_STOP; break; }
+                    if (float32_overflows(current.value)) { error("strconv.ParseFloat: parsing " + obm::go_quote(current.value) + ": value out of range"); st = S_STOP; break; }
                     if (!set_argument(arg, 2, current.value)) { st = S_STOP; break; }
                     args.push_back(Arg{arg, 2, current.value});
                 } else if (consumed(OBM_K_STRING_LITERAL)) {
@@ -475,8 +460,8 @@ extern "C" int64_t obm_results_format_doc(const obm_registry *reg, const uint8_t
         } else { /* error.go:8-22: "<msg>, on marker <name> at {line:L column:C}" */
             const obm_arg &g = args_base[r.arg_base];
             const std::string v((const char *)doc + g.val_off, g.val_len);
-            std::string m = (r.flags & OBM_R_ERR_PARSEBOOL) ? "strconv.ParseBool: parsing " + go_quote_simple(v) + ": invalid syntax"
-                                                             : "strconv.ParseFloat: parsing " + go_quote_simple(v) + ": value out of range";
+            std::string m = (r.flags & OBM_R_ERR_PARSEBOOL) ? "strconv.ParseBool: parsing " + obm::go_quote(v) + ": invalid syntax"
+                                                             : "strconv.ParseFloat: parsing " + obm::go_quote(v) + ": value out of range";
             char pos[96]; snprintf(pos, sizeof pos, "{line:%u column:%u}", g.name_off, r.aux);
             m += ", on marker " + d.name + " at " + pos;
             o.push_back(1); put_u32(o, (uint32_t)m.size()); o += m; put_u32(o, (uint32_t)text.size()); o += text;

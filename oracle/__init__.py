@@ -59,8 +59,27 @@ def lib():
         L.obo_atoi_err.argtypes = [ctypes.c_char_p, ctypes.c_uint64]
         L.obo_quote.argtypes = [ctypes.c_char_p, ctypes.c_uint64, ctypes.c_char_p, ctypes.c_uint64]
         L.obo_quote.restype = ctypes.c_uint64
+        L.obo_classify.argtypes = [ctypes.c_void_p, ctypes.c_uint64, ctypes.c_void_p]
         _LIB = L
     return _LIB
+
+
+def quote(b: bytes) -> bytes:
+    """strconv.Quote of a byte string (Go 1.16, Unicode 13.0 IsPrint)"""
+    L = lib()
+    n = L.obo_quote(b, len(b), None, 0)
+    out = ctypes.create_string_buffer(n)
+    L.obo_quote(b, len(b), out, n)
+    return out.raw
+
+
+def classify(cps):
+    """int32 code points -> uint8 bits: 1 unicode.IsLetter, 2 IsNumber, 4 IsSpace, 8 strconv.IsPrint"""
+    import numpy as np
+    cps = np.ascontiguousarray(cps, dtype=np.int32)
+    out = np.zeros(len(cps), dtype=np.uint8)
+    lib().obo_classify(cps.ctypes.data, len(cps), out.ctypes.data)
+    return out
 
 
 def generate_corpus(ndocs: int, doc_bytes: int = 4096, first_doc: int = 0, flavour: int = 0):

@@ -14,8 +14,8 @@
  * is not vendored under /root/reference and cannot be built here (no Go toolchain):
  *   bufio.Reader  (default 4096-byte buffer; Peek/Discard/ReadRune/UnreadRune)  -> bufreader_* below,
  *   unicode/utf8  (DecodeRune, RuneLen)                                          -> go_decode_rune, go_rune_len,
- *   unicode       (IsSpace/IsLetter/IsNumber, Unicode 13.0 tables)               -> go_unicode_tables.h (see its header
- *                                                                                  for the post-13.0 caveat),
+ *   unicode       (IsSpace/IsLetter/IsNumber, Unicode 13.0 tables)               -> go_unicode_tables.h (generated from
+ *                                                                                  tests/golden/unicode13.json),
  *   strconv       (ParseFloat(.,64), Atoi, Quote)                                -> go_parse_float_err, go_atoi_err, go_quote,
  *   fmt           (%s %q %d %+v of the shapes used in error.go / state.go)       -> hand formatted.
  * Those are restated from their published behaviour.
@@ -964,4 +964,11 @@ int obo_atoi_err(const uint8_t *s, uint64_t n) { return go_atoi_err(s, (size_t)n
 uint64_t obo_quote(const uint8_t *s, uint64_t n, uint8_t *out, uint64_t cap) {
     gstr o = {0}; go_quote(&o, s, (size_t)n);
     uint64_t len = o.len; memcpy(out, o.p, len < cap ? len : cap); gs_free(&o); return len;
+}
+/* out[i] bit 0: unicode.IsLetter, bit 1: IsNumber, bit 2: IsSpace, bit 3: strconv.IsPrint of cps[i] */
+void obo_classify(const int32_t *cps, uint64_t n, uint8_t *out) {
+    for (uint64_t i = 0; i < n; i++) {
+        int32_t r = cps[i];
+        out[i] = (uint8_t)(go_is_letter(r) | go_is_number(r) << 1 | go_is_space(r) << 2 | go_is_print(r) << 3);
+    }
 }

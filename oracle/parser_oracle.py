@@ -67,27 +67,11 @@ def read_float_magnitude(v: bytes) -> Decimal:
 
 
 def go_quote(b: bytes) -> str:
-    """strconv.Quote for the values that can reach a strconv error here (printable ASCII + whitespace)."""
-    out = ['"']
-    for ch in b.decode("utf-8", "replace"):
-        if ch in '"\\':
-            out.append("\\" + ch)
-        elif ch == "\n":
-            out.append("\\n")
-        elif ch == "\t":
-            out.append("\\t")
-        elif ch == "\r":
-            out.append("\\r")
-        elif ch == "\v":
-            out.append("\\v")
-        elif ch == "\f":
-            out.append("\\f")
-        elif ord(ch) < 0x20 or ord(ch) == 0x7F:
-            out.append("\\x%02x" % ord(ch) if ord(ch) < 0x20 else "\\u007f")
-        else:
-            out.append(ch)
-    out.append('"')
-    return "".join(out)
+    """strconv.Quote: the lexer oracle's (lexer_oracle.c go_quote, Unicode 13.0 IsPrint), so that both oracles quote alike.
+    Values reach it with white space of any kind (consumedWhitespaced takes Unicode white space into a bool literal) and
+    with any text (a FieldType value)."""
+    from oracle import quote
+    return quote(b).decode("utf-8")
 
 
 class Parser:

@@ -23,6 +23,8 @@ def build(force=False):
             os.path.join(_ROOT, "operator-builder_b200", "csrc", "obm_warp_core.h"),
             os.path.join(_HERE, "warp_emu.h"),
             os.path.join(_ROOT, "operator-builder_b200", "csrc", "obm_parse_dev.h"),
+            os.path.join(_ROOT, "operator-builder_b200", "csrc", "obm_quote.h"),
+            os.path.join(_ROOT, "operator-builder_b200", "csrc", "go_unicode_tables.h"),
             os.path.join(_ROOT, "include", "obmarkers.h")]
     if force or not os.path.exists(so) or any(os.path.getmtime(s) > os.path.getmtime(so) for s in srcs):
         subprocess.check_call(["g++", "-O2", "-g", "-std=c++17", "-fPIC", "-Wall", "-Wextra", "-Wno-unknown-pragmas", *(["-DOBMW_DEBUG"] if os.environ.get("OBMW_DEBUG") else []), "-shared", "-o", so,
@@ -63,6 +65,22 @@ def lib():
         L.obm_decode_doc.argtypes = [ctypes.c_char_p, ctypes.c_uint64, ctypes.c_void_p, ctypes.c_uint64,
                                      ctypes.POINTER(ctypes.POINTER(ctypes.c_uint8)), ctypes.POINTER(ctypes.c_uint64)]
         L.obm_free.argtypes = [ctypes.c_void_p]
+        L.hs_classify.argtypes = [ctypes.c_void_p, ctypes.c_uint64, ctypes.c_void_p]
+        L.hs_go_quote.restype = ctypes.c_uint64
+        L.hs_go_quote.argtypes = [ctypes.c_char_p, ctypes.c_uint64, ctypes.c_char_p, ctypes.c_uint64]
+        u8pp = ctypes.POINTER(ctypes.POINTER(ctypes.c_uint8))
+        L.hs_lex_decode_batch.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_uint32, u8pp, ctypes.POINTER(ctypes.c_uint64),
+                                          ctypes.c_void_p, ctypes.c_void_p]
+        L.hs_decode_batch.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_uint32, ctypes.c_void_p, ctypes.c_void_p, u8pp,
+                                      ctypes.POINTER(ctypes.c_uint64), ctypes.c_void_p]
+        # the parser (obm_parse.cpp) over the host tables, with registries of this library's own
+        L.obm_registry_new.restype = ctypes.c_void_p
+        L.obm_registry_free.argtypes = [ctypes.c_void_p]
+        L.obm_registry_add.argtypes = [ctypes.c_void_p, ctypes.c_char_p, ctypes.POINTER(ctypes.c_char_p), ctypes.c_uint32]
+        L.obm_registry_define.argtypes = [ctypes.c_void_p, ctypes.c_int]
+        L.obm_parse_doc.restype = ctypes.c_int64
+        L.obm_parse_doc.argtypes = [ctypes.c_void_p, ctypes.c_char_p, ctypes.c_uint64, ctypes.c_void_p, ctypes.c_uint64, u8pp,
+                                    ctypes.POINTER(ctypes.c_uint64)]
         _LIB = L
     return _LIB
 
@@ -112,6 +130,81 @@ def decode(doc: bytes, tuples, L=None) -> bytes:
     data = ctypes.string_at(out, outlen.value)
     L.obm_free(out)
     return data
+
+
+def classify(cps):
+    """int32 code points -> uint8 bits of the product's host classes: 1 is_letter, 2 is_number, 4 is_space, 8 go_is_print"""
+    cps = np.ascontiguousarray(cps, dtype=np.int32)
+    out = np.zeros(len(cps), dtype=np.uint8)
+    lib().hs_classify(cps.ctypes.data, len(cps), out.ctypes.data)
+    return out
+
+
+def go_quote(b: bytes) -> bytes:
+    """the product's strconv.Quote (csrc/obm_quote.h)"""
+    L = lib()
+    n = L.hs_go_quote(b, len(b), None, 0)
+    out = ctypes.create_string_buffer(n)
+    L.hs_go_quote(b, len(b), out, n)
+    return out.raw
+
+
+def _take(out, outlen):
+    data = ctypes.string_at(out, outlen.value)
+    lib().obm_free(out)
+    return data
+
+
+def lex_decode_batch(data, doc_off):
+    """host exact lexer + obm_decode_doc over a packed batch -> (stream bytes, stream_off uint64[ndocs+1], lexemes
+    uint64[ndocs]), the layout of oracle.lex_batch_raw"""
+    L = lib()
+    doc_off = np.ascontiguousarray(doc_off, dtype=np.uint64)
+    ndocs = len(doc_off) - 1
+    out, outlen = ctypes.POINTER(ctypes.c_uint8)(), ctypes.c_uint64()
+    soff, nlex = np.zeros(ndocs + 1, dtype=np.uint64), np.zeros(ndocs, dtype=np.uint64)
+    assert L.hs_lex_decode_batch(data.ctypes.data, doc_off.ctypes.data, ndocs, ctypes.byref(out), ctypes.byref(outlen),
+                                 soff.ctypes.data, nlex.ctypes.data) == 0
+    return _take(out, outlen), soff, nlex
+
+
+def decode_batch(data, doc_off, tuples, tuple_off):
+    """obm_decode_doc of every document of a batch from its tuples -> (stream bytes, stream_off uint64[ndocs+1])"""
+    L = lib()
+    doc_off = np.ascontiguousarray(doc_off, dtype=np.uint64)
+    tuples = np.ascontiguousarray(tuples, dtype=np.uint64)
+    tuple_off = np.ascontiguousarray(tuple_off, dtype=np.uint64)
+    ndocs = len(doc_off) - 1
+    out, outlen = ctypes.POINTER(ctypes.c_uint8)(), ctypes.c_uint64()
+    soff = np.zeros(ndocs + 1, dtype=np.uint64)
+    assert L.hs_decode_batch(data.ctypes.data, doc_off.ctypes.data, ndocs, tuples.ctypes.data, tuple_off.ctypes.data,
+                             ctypes.byref(out), ctypes.byref(outlen), soff.ctypes.data) == 0
+    return _take(out, outlen), soff
+
+
+class Registry:
+    """an obm_registry of this library (names only: {marker: [args]}, or typed: define=[marker types])"""
+
+    def __init__(self, markers=None, define=()):
+        self._L = lib()
+        self.handle = self._L.obm_registry_new()
+        for name, args in (markers or {}).items():
+            arr = (ctypes.c_char_p * max(1, len(args)))(*args)
+            self._L.obm_registry_add(self.handle, name, arr, len(args))
+        for t in define:
+            assert self._L.obm_registry_define(self.handle, t) == 0
+
+    def __del__(self):
+        self._L.obm_registry_free(self.handle)
+
+
+def parse_doc(registry, doc: bytes) -> bytes:
+    """obm_parse_doc over the host exact lexer's tuples of one document -> serialised Results"""
+    L = lib()
+    t = lex_doc(doc)
+    out, outlen = ctypes.POINTER(ctypes.c_uint8)(), ctypes.c_uint64()
+    assert L.obm_parse_doc(registry.handle, doc, len(doc), t.ctypes.data, len(t), ctypes.byref(out), ctypes.byref(outlen)) >= 0
+    return _take(out, outlen)
 
 
 def fmt_tuples(tuples):

@@ -45,6 +45,88 @@ int hs_atoi_err(const uint8_t *s, uint32_t n) { return obm::atoi_err(s, n); }
 }
 
 /* ---------------------------------------------------------------------------------------------
+ * Unicode hooks (tests/test_unicode13.py): the product's classes and quoter over the host tables, and
+ * batch lex + decode in the record format of the oracle's obo_lex_batch, so that millions of one-line
+ * documents compare as one byte string.
+ * ------------------------------------------------------------------------------------------- */
+#include <string>
+#include <vector>
+#include "../../include/obmarkers.h"
+#include "../../operator-builder_b200/csrc/obm_quote.h"
+
+namespace {
+/* obm_decode_doc of one document appended to `out` -> its lexeme count */
+int64_t decode_append(std::string &out, const uint8_t *doc, uint64_t n, const obm_tuple *t, uint64_t nt) {
+    uint8_t *p = nullptr; uint64_t len = 0;
+    int64_t c = obm_decode_doc(doc, n, t, nt, &p, &len);
+    if (c < 0) return c;
+    out.append((const char *)p, len);
+    free(p);
+    return c;
+}
+/* the serialised batch handed to the caller (release with obm_free) */
+int finish(const std::string &buf, uint8_t **out, uint64_t *out_len) {
+    uint8_t *p = (uint8_t *)malloc(buf.size() ? buf.size() : 1);
+    if (!p) return OBM_E_NOMEM;
+    memcpy(p, buf.data(), buf.size());
+    *out = p; *out_len = buf.size();
+    return 0;
+}
+} // namespace
+
+extern "C" {
+/* out[i] bit 0: obm::is_letter, bit 1: obm::is_number, bit 2: obm::is_space, bit 3: obm::go_is_print (strconv.IsPrint) */
+void hs_classify(const int32_t *cps, uint64_t n, uint8_t *out) {
+    for (uint64_t i = 0; i < n; i++) {
+        const int r = cps[i];
+        out[i] = (uint8_t)(obm::is_letter(TBL, r) | obm::is_number(TBL, r) << 1 | obm::is_space(r) << 2 | obm::go_is_print(r) << 3);
+    }
+}
+/* strconv.Quote of s as the decoder and the parser print it; returns the full length (writes at most cap) */
+uint64_t hs_go_quote(const uint8_t *s, uint64_t n, uint8_t *out, uint64_t cap) {
+    const std::string q = obm::go_quote(std::string((const char *)s, n));
+    memcpy(out, q.data(), q.size() < cap ? q.size() : cap);
+    return q.size();
+}
+/* every document through the host build of the exact lexer, then obm_decode_doc: stream_off[ndocs+1] and n_lexemes[ndocs]
+ * as obo_lex_batch fills them */
+int hs_lex_decode_batch(const uint8_t *bytes, const uint64_t *doc_off, uint32_t ndocs, uint8_t **out, uint64_t *out_len,
+                        uint64_t *stream_off, uint64_t *n_lexemes) {
+    std::string buf;
+    std::vector<obm_tuple> t;
+    for (uint32_t d = 0; d < ndocs; d++) {
+        const uint8_t *doc = bytes + doc_off[d];
+        const uint32_t n = (uint32_t)(doc_off[d + 1] - doc_off[d]);
+        uint64_t nt = 2 * (uint64_t)n + 16;
+        for (;;) {
+            t.resize(nt);
+            const uint64_t got = hs_lex_doc(doc, n, t.data(), nt, nullptr, nullptr);
+            if (got <= nt) { nt = got; break; }
+            nt = got;
+        }
+        stream_off[d] = buf.size();
+        const int64_t c = decode_append(buf, doc, n, t.data(), nt);
+        if (c < 0) return (int)c;
+        n_lexemes[d] = (uint64_t)c;
+    }
+    stream_off[ndocs] = buf.size();
+    return finish(buf, out, out_len);
+}
+/* obm_decode_doc over given tuples: document d's are tuples[tuple_off[d] .. tuple_off[d+1]) */
+int hs_decode_batch(const uint8_t *bytes, const uint64_t *doc_off, uint32_t ndocs, const obm_tuple *tuples, const uint64_t *tuple_off,
+                    uint8_t **out, uint64_t *out_len, uint64_t *stream_off) {
+    std::string buf;
+    for (uint32_t d = 0; d < ndocs; d++) {
+        stream_off[d] = buf.size();
+        const int64_t c = decode_append(buf, bytes + doc_off[d], doc_off[d + 1] - doc_off[d], tuples + tuple_off[d], tuple_off[d + 1] - tuple_off[d]);
+        if (c < 0) return (int)c;
+    }
+    stream_off[ndocs] = buf.size();
+    return finish(buf, out, out_len);
+}
+}
+
+/* ---------------------------------------------------------------------------------------------
  * CTA emulation of the tile fast path (obm_fast.cuh's k_tile_scan): the same phase functions from
  * obm_tile.h, run for tid = 0..NT-1 between "barriers", tiles visited in order (which is what the
  * look-back chain enforces on the device).
