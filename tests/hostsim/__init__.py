@@ -52,6 +52,10 @@ def lib():
         L.hs_warp_batch_report.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_uint32, ctypes.c_void_p, ctypes.c_uint64,
                                            ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_uint64,
                                            ctypes.POINTER(ctypes.c_uint64)]
+        L.hs_warp_line_stats.argtypes = [ctypes.POINTER(ctypes.c_uint64), ctypes.POINTER(ctypes.c_uint64)]
+        L.hs_fast_lines.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_uint32, ctypes.c_void_p, ctypes.c_void_p,
+                                    ctypes.c_uint64, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_uint64, ctypes.c_void_p,
+                                    ctypes.c_void_p]
         L.hs_warp_units.restype = ctypes.c_uint64
         L.hs_warp_units.argtypes = [ctypes.c_void_p, ctypes.c_uint32]
         L.hs_large_doc.restype = ctypes.c_uint64
@@ -270,6 +274,40 @@ def warp_batch(docs, skew=0):
     assert n != BAD_STARTS, "the warp replay's document starts differ from doc_off"
     assert n <= cap and nu.value == rcap
     return out[:n].copy(), toff, stats, report
+
+
+def warp_line_stats():
+    """(marker lines the fused warp kernel's phase C stepper took, lines it handed to the generic lexer) over every
+    hs_warp_batch* call of this process so far"""
+    fast, generic = ctypes.c_uint64(), ctypes.c_uint64()
+    lib().hs_warp_line_stats(ctypes.byref(fast), ctypes.byref(generic))
+    return fast.value, generic.value
+
+
+# one row per document of fast_lines
+FAST_LINES = np.dtype([(f, np.uint32) for f in ("res", "lines", "ok", "ovf", "max_tuples", "max_len")])
+FLR_OK, FLR_FALLBACK, FLR_NONE = 0, 1, 2
+
+
+def fast_lines(data, doc_off, skews):
+    """The phase C stepper (obmw::fast_line) on every marker line of each document of a packed batch, the document copied
+    to skews[d] bytes past a 16-byte boundary (hs_fast_lines) -> (info, direct, toff, staged, soff): info[d] (FAST_LINES)
+    says how document d went; direct[toff[d]:toff[d+1]] are its tuples with EOF (DirectSink), empty when a line was handed
+    to the generic lexer; staged[soff[d]:soff[d+1]] the same from the PackSink, empty also when a line overflowed it"""
+    L = lib()
+    data = np.ascontiguousarray(data, dtype=np.uint8)
+    off = np.ascontiguousarray(doc_off, dtype=np.uint64)
+    skews = np.ascontiguousarray(skews, dtype=np.uint8)
+    ndocs = len(off) - 1
+    assert len(skews) == ndocs
+    cap = 2 * int(off[-1]) + 4 * ndocs + 16
+    direct, staged = np.zeros(cap, dtype=np.uint64), np.zeros(cap, dtype=np.uint64)
+    toff, soff = np.zeros(ndocs + 1, dtype=np.uint64), np.zeros(ndocs + 1, dtype=np.uint64)
+    info = np.zeros(ndocs, dtype=FAST_LINES)
+    rc = L.hs_fast_lines(data.ctypes.data, off.ctypes.data, ndocs, skews.ctypes.data, direct.ctypes.data, cap, toff.ctypes.data,
+                         staged.ctypes.data, cap, soff.ctypes.data, info.ctypes.data)
+    assert rc == 0, rc
+    return info, direct[:int(toff[-1])], toff, staged[:int(soff[-1])], soff
 
 
 def warp_units(doc_off):

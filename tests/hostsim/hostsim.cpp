@@ -729,6 +729,94 @@ extern "C" uint64_t hs_warp_batch(const uint8_t *bytes, const uint64_t *doc_off,
     (void)fake_skew; /* the skew is the batch's address (tests/hostsim/__init__.py) */
     return hs_warp_batch_report(bytes, doc_off, ndocs, out, cap, tuple_off, stats, nullptr, 0, nullptr);
 }
+/* ---------------------------------------------------------------------------------------------
+ * The phase C stepper alone (tests/test_marker_lines.py): obmw::fast_line on every marker line of each document, from a
+ * 16-byte aligned buffer that holds the document at its skew with the staged text's 16 bytes of slack behind it (BUFB -
+ * MAXDOC), poisoned around.  The owning lines, their first special ('#', "//" or '+') and first '+' are found as phase B
+ * finds them, by a plain byte loop instead of the bitmaps; a '+' PD_GENERIC or more bytes after the first special is the
+ * generic lexer's, as in the kernel.  Every marker line runs once into a DirectSink and once into a PackSink(cap = LTS).
+ * Per document, out of info[6 * d ...]:
+ *   [0] FLR_OK: every marker line on the stepper; FLR_FALLBACK: at least one handed over; FLR_NONE: no marker line
+ *   [1] marker lines, [2] of them on the stepper, [3] some stepper line overflowed its PackSink (ovf)
+ *   [4] most tuples of one stepper line, [5] largest len of a stepper line's DirectSink tuples
+ * direct[toff[d] .. toff[d+1]): the document's tuples (stepper lines from the DirectSink, plain comment lines as phase D
+ * writes them) and EOF -- empty when a line was handed over.  staged[soff[d] .. soff[d+1]): the same with the stepper
+ * lines' PackSink tuples unpacked -- empty when a line was handed over or overflowed.  Returns 0, or -1 when a document
+ * is longer than MAXDOC or an output is too small.
+ * ------------------------------------------------------------------------------------------- */
+enum { FLR_OK = 0, FLR_FALLBACK = 1, FLR_NONE = 2 };
+extern "C" int hs_fast_lines(const uint8_t *bytes, const uint64_t *doc_off, uint32_t ndocs, const uint8_t *skews, obm_tuple *direct,
+                             uint64_t dcap, uint64_t *toff, obm_tuple *staged, uint64_t scap, uint64_t *soff, uint32_t *info) {
+    using namespace obmw;
+    alignas(16) static uint8_t buf[BUFB + 64];
+    uint32_t pk[LTS];
+    uint64_t at = 0, sat = 0;
+    toff[0] = 0; soff[0] = 0;
+    for (uint32_t d = 0; d < ndocs; d++) {
+        const uint32_t n = (uint32_t)(doc_off[d + 1] - doc_off[d]);
+        const uint32_t skew = skews[d] & 15u;
+        if (n > MAXDOC) return -1;
+        for (size_t i = 0; i < sizeof buf; i++) buf[i] = POISON[(i + d) % sizeof POISON];
+        memcpy(buf + skew, bytes + doc_off[d], n);
+        const uint8_t *t = buf;
+        const uint32_t dpos = skew, dend = skew + n;
+        uint32_t *inf = info + 6ull * d;
+        memset(inf, 0, 6 * sizeof(uint32_t));
+        bool fell = false, ovf = false;
+        const uint64_t at0 = at, sat0 = sat;
+        auto put2 = [&](uint32_t kind, uint32_t off, uint32_t len) {
+            if (at < dcap) direct[at] = OBM_TUPLE(kind, off, len);
+            if (sat < scap) staged[sat] = OBM_TUPLE(kind, off, len);
+            at++; sat++;
+        };
+        for (uint32_t ls = dpos, line = 1; ls < dend; line++) {
+            uint32_t le = ls;
+            while (le < dend && t[le] != '\n') le++;
+            uint32_t first = ls;
+            while (first < le && !(t[first] == '#' || t[first] == '+' || (t[first] == '/' && first + 1 < dend && t[first + 1] == '/'))) first++;
+            if (first < le) {
+                uint32_t plus = first;
+                while (plus < le && t[plus] != '+') plus++;
+                if (plus < le) { /* a marker line */
+                    inf[1]++;
+                    uint32_t res = FL_FALLBACK;
+                    if (plus - first < PD_GENERIC) {
+                        const uint64_t room = at < dcap ? dcap - at : 0;
+                        DirectSink ds(direct + at, room < 0xFFFFFFFFull ? (uint32_t)room : 0xFFFFFFFFu);
+                        res = fast_line(t, first, plus, ls, line, dpos, dend, ds);
+                        PackSink ps(pk, LTS);
+                        const uint32_t res2 = fast_line(t, first, plus, ls, line, dpos, dend, ps);
+                        if (res2 != res || ps.n != ds.n || ps.mk != ds.mk || ps.lx != ds.lx) return -2; /* the sinks are passive */
+                        if (res == FL_OK) {
+                            inf[2]++;
+                            if (ds.n > inf[4]) inf[4] = ds.n;
+                            for (uint32_t k = 0; k < ds.n && at + k < dcap; k++) {
+                                const uint32_t len = (uint32_t)((direct[at + k] >> 32) & 0x7FFFFFFu);
+                                if (len > inf[5]) inf[5] = len;
+                            }
+                            ovf |= ps.ovf;
+                            if (!ps.ovf) for (uint32_t k = 0; k < ps.n; k++) { if (sat + k < scap) staged[sat + k] = st_unpack(pk[k]); }
+                            at += ds.n; sat += ps.n;
+                        }
+                    }
+                    fell |= res != FL_OK;
+                } else { /* a plain comment line */
+                    if (line != 1) put2(OBM_K_LINE, ls - dpos, line);
+                    put2(OBM_K_COMMENT, first - dpos, t[first] == '/' ? 2 : 1);
+                }
+            }
+            ls = le + 1;
+        }
+        put2(OBM_K_EOF, n, 0);
+        inf[0] = fell ? FLR_FALLBACK : inf[1] ? FLR_OK : FLR_NONE;
+        inf[3] = ovf;
+        if (fell) at = at0;
+        if (fell || ovf) sat = sat0;
+        toff[d + 1] = at; soff[d + 1] = sat;
+    }
+    return at <= dcap && sat <= scap ? 0 : -1;
+}
+
 /* units of the batch (k_wunits + the scan): what k_warp_scan's warps share */
 extern "C" uint64_t hs_warp_units(const uint64_t *doc_off, uint32_t ndocs) {
     const uint64_t ntiles = doc_off[ndocs] / obmw::TILE + 1;
