@@ -670,11 +670,17 @@ static int obm_pipe_launch(obm_handle *h, const uint8_t *d_bytes, const uint64_t
 /* ---- fused warp kernel (mode 0) ----------------------------------------------------------------------- */
 static uint64_t warp_ntiles(uint64_t total_bytes) { return total_bytes / obmw::TILE + 1; }
 static uint64_t warp_units_max(uint32_t ndocs, uint64_t total_bytes) { return 2 * warp_ntiles(total_bytes) + ndocs / obmw::DMAX + 2; }
+/* k_warp_scan's grid cap for a batch: no more warps than units, no more CTAs than MAX_CTAS (the launch takes the smaller of
+ * this and the device's resident CTAs) */
+static uint64_t warp_max_ctas(uint64_t um) { const uint64_t c = (um + obmw::WPC - 1) / obmw::WPC; return c < obmw::MAX_CTAS ? c : obmw::MAX_CTAS; }
+/* the warps' fin slots live in the call's scratch, not in the handle: obm_lex_batch / obm_parse_batch run the scans of
+ * different chunks concurrently, each with its own scratch */
+static uint64_t warp_fin_bytes(uint64_t um) { return warp_max_ctas(um) * obmw::WPC * obmw::FIN_CAP * sizeof(uint32_t); }
 static uint64_t warp_scratch_bytes(uint32_t ndocs, uint64_t total_bytes) {
     const uint64_t nt = warp_ntiles(total_bytes), um = warp_units_max(ndocs, total_bytes);
     return align_up((nt + 2) * 4, 256) + align_up((obm_fast_max_large(total_bytes) + 1) * 4, 256) + align_up(nt * 4 + 4, 256) + align_up((nt + 1) * 8, 256) +
            align_up(((uint64_t)scan_tiles((uint32_t)nt) + 1) * 8, 256) + align_up((nt + 1) * sizeof(obmw::WRec), 256) + align_up((um + 1) * 8, 256) +
-           align_up(2 * (um / 32 + 2) * 8, 256) + align_up((um + 1) * sizeof(obmw::WUnit), 256) + 512;
+           align_up(2 * (um / 32 + 2) * 8, 256) + align_up((um + 1) * sizeof(obmw::WUnit), 256) + align_up(warp_fin_bytes(um), 256) + 512;
 }
 /* tile index -> (large documents planned and counted on a side stream) units per tile + scan -> k_warp_scan -> fill of
  * the large documents */
@@ -698,6 +704,7 @@ static int obm_warp_launch(obm_handle *h, const uint8_t *d_bytes, const uint64_t
     obmw::WUnit *units = (obmw::WUnit *)q; q += up((um + 1) * sizeof(obmw::WUnit));
     obmw::WArgs A;
     A.units = units;
+    A.fin_slots = (uint32_t *)q; q += up(warp_fin_bytes(um));
     A.bytes = d_bytes; A.doc_off = d_doc_off; A.ndocs = ndocs; A.total_bytes = total_bytes; A.tile_first = tile_first; A.ntiles = ntiles;
     A.ubase = ubase;
     A.st_tuples = (uint64_t *)q; q += up((um + 1) * 8);
@@ -721,7 +728,7 @@ static int obm_warp_launch(obm_handle *h, const uint8_t *d_bytes, const uint64_t
     OBM_CUDA(h, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, obmw::k_warp_scan, (int)(obmw::WPC * 32), smem));
     if (per_sm < 1) per_sm = 1;
     uint32_t grid = (uint32_t)dev_sms * (uint32_t)per_sm; /* persistent warps: a multiple of the SM count */
-    const uint32_t gmax = (uint32_t)((um < 0xFFFFFFF0ull ? um : 0xFFFFFFF0ull) + obmw::WPC - 1) / obmw::WPC;
+    const uint32_t gmax = (uint32_t)warp_max_ctas(um); /* the fin slots are carved for this many CTAs */
     if (grid > gmax) grid = gmax;
     OBM_CUDA(h, cudaStreamWaitEvent(st, h->ev_join, 0));
     obmw::k_warp_scan<<<grid, obmw::WPC * 32, smem, st>>>(A);

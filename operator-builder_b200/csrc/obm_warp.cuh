@@ -19,13 +19,20 @@
 #define WSYNC() __syncwarp()
 #define WTEXT(S) obm::ShBytes{obmf::smem_u32((S).text), (S).text}
 #define WATOMIC_OR(p, v) atomicOr((p), (v))
+#define OBMW_FIN_GLOBAL /* W.fin is a slot in global memory: see WarpSmem */
 #include "obm_warp_core.h"
+
+#ifndef OBMW_WPC
+#define OBMW_WPC 11
+#endif
 
 namespace obmw {
 
-constexpr uint32_t WPC = 10; /* warps per CTA; each works alone on its own shared-memory slice and never meets the others (no barrier).  10 = every
-                              * warp the SM's 227 KB of shared memory holds (23.2 KB each), as ONE CTA so that the CTA's warps are dealt round-robin
-                              * to the SM's four schedulers (single-warp CTAs are not) */
+constexpr uint32_t WPC = OBMW_WPC; /* warps per CTA; each works alone on its own shared-memory slice and never meets the others (no barrier).  11 =
+                                    * every warp the SM's 227 KB of shared memory holds (20.4 KB each, fin in global memory), as ONE CTA so that the
+                                    * CTA's warps are dealt round-robin to the SM's four schedulers (single-warp CTAs are not) */
+constexpr uint32_t MAX_CTAS = 256; /* grid cap of k_warp_scan (>= the SM count of any H100): the call's scratch holds this many CTAs' fin slots
+                                    * without depending on the device it runs on */
 enum { WC_TICKET = 0 };
 #ifdef OBMW_PHASE_CLOCKS
 __device__ unsigned long long g_phase_cycles[PC_N + 1]; /* cycles per bucket summed over warps; [PC_N]: units */
@@ -138,12 +145,15 @@ __device__ __forceinline__ uint64_t chain_resolve(uint64_t *st_units, uint64_t *
  * write unit i-1 from W.fin (its exclusive prefix has had a whole unit's time to arrive: no waiting on the chain),
  * assemble unit i into W.fin, scan unit i+1 ...  A unit whose write needs the staged text (documents for the exact
  * lexer, marker lines that are not staged) or that does not fit W.fin is written at once instead. */
-__global__ void __launch_bounds__(WPC * 32, 1) /* one CTA per SM: ptxas may take the registers it wants (151 on sm_90a; without the hint it settles for fewer and spills) */
+__global__ void __launch_bounds__(WPC * 32, 1) /* one CTA per SM: ptxas may take the registers it wants (up to 184 at 11 warps; without the hint it settles for fewer and spills) */
 k_warp_scan(WArgs A) {
     extern __shared__ __align__(16) uint8_t smem_raw[];
     WarpSmem &S = reinterpret_cast<WarpSmem *>(smem_raw)[threadIdx.x >> 5];
     const uint32_t lane = threadIdx.x & 31u;
-    if (lane == 0) { obmf::mbar_init(&S.mbar, 1); obmf::fence_mbar_init(); }
+    if (lane == 0) {
+        obmf::mbar_init(&S.mbar, 1); obmf::fence_mbar_init();
+        S.fin = A.fin_slots + (size_t)(blockIdx.x * WPC + (threadIdx.x >> 5)) * FIN_CAP; /* the warp's own slot (grid <= MAX_CTAS) */
+    }
     __syncwarp();
     const obm::Tables T = obmq::dev_tables();
     const uint32_t nunits = (uint32_t)A.ubase[A.ntiles];
@@ -193,9 +203,11 @@ k_warp_scan(WArgs A) {
         }
         OBMW_PC_MARK(PC_OTHER);
         if (have_pend) {
+            FinRegs F;
+            fin_load(S, A, pend, F); /* the slot's round trip overlaps the chain's */
             const uint64_t base = chain_resolve(A.st_tuples, A.st_blocks, pend.u, nblocks);
             OBMW_PC_MARK(PC_CHAIN);
-            write_fin(S, A, pend, nunits, base);
+            write_fin(A, pend, nunits, base, F);
             OBMW_PC_MARK(PC_WRITE);
             have_pend = false;
         }
@@ -213,9 +225,11 @@ k_warp_scan(WArgs A) {
 #endif
     }
     if (have_pend) {
+        FinRegs F;
+        fin_load(S, A, pend, F);
         const uint64_t base = chain_resolve(A.st_tuples, A.st_blocks, pend.u, nblocks);
         OBMW_PC_MARK(PC_CHAIN);
-        write_fin(S, A, pend, nunits, base);
+        write_fin(A, pend, nunits, base, F);
         OBMW_PC_MARK(PC_WRITE);
     }
 #ifdef OBMW_PHASE_CLOCKS

@@ -59,8 +59,15 @@ struct UnitSet {
 struct WarpSmem {
     alignas(16) uint8_t text[BUFB + 64];
     UnitSet set;
-    uint32_t fin[FIN_CAP];      /* the unit's tuples, packed (st_pack), in final order: what the DEFERRED write needs -- a warp scans
-                                 * its next unit while this unit's tuple count travels through the chain (obm_warp.cuh) */
+    /* the unit's tuples, packed (st_pack), in final order: what the DEFERRED write needs -- a warp scans its next unit while
+     * this unit's tuple count travels through the chain (obm_warp.cuh).  Phases A-C never read it, so the device build
+     * (OBMW_FIN_GLOBAL) keeps it in a per-warp slot of FIN_CAP words in global memory (WArgs::fin_slots), which an L2 of
+     * 50 MB holds easily: the 2.75 KiB it would take here are what lets an SM hold an eleventh warp */
+#ifdef OBMW_FIN_GLOBAL
+    uint32_t *fin;
+#else
+    uint32_t fin[FIN_CAP];
+#endif
     uint16_t nlpre[NWORDS / 2]; /* newline bits in words [0, 2k): every second word, the odd ones add their neighbour's count */
     uint32_t naw[NWORDS / 32 + 1]; /* per row: the 32-byte words that hold bytes >= 0x80 */
     uint32_t dstart[DMAX + 2];  /* document starts, buffer-relative; [nd] = end */
@@ -91,6 +98,7 @@ struct WArgs {
     const uint32_t *counts;                  /* tuple counts of large documents (k_large_resolve) */
     obm_tuple *out; uint64_t out_cap; uint64_t *tuple_off;
     uint32_t *status; unsigned long long *totals; uint32_t *ctl;
+    uint32_t *fin_slots;                     /* OBMW_FIN_GLOBAL: FIN_CAP words per warp of the grid, warp w of CTA b at (b * WPC + w) * FIN_CAP */
 };
 /* where a unit's text lies: computed ahead of the unit so that its bulk copy can be issued early.  doff: doc_off[da + lane]
  * on lanes 0..nd once the caller has loaded it with the prestaged copy (compute_unit loads it otherwise) */
@@ -546,15 +554,16 @@ OBMW_DEV bool assemble_fin(WarpSmem &W, UnitSet &S, const UnitRegs &R, WAcc &acc
     const uint32_t lane = WLANE();
     const uint32_t nd = R.nd, n_owners = R.n_owners, n_ml = R.n_ml;
     if (R.n_small > FIN_CAP || R.long_line) return false;
-    if (lane < nd) { W.fin[R.dexcl + R.dtot - 1u] = st_pack(OBM_K_EOF, R.dlen, 0); acc.lexemes++; }
+    uint32_t *const fin = W.fin; /* one read of the slot pointer (OBMW_FIN_GLOBAL), not one per store */
+    if (lane < nd) { fin[R.dexcl + R.dtot - 1u] = st_pack(OBM_K_EOF, R.dlen, 0); acc.lexemes++; }
     for (uint32_t o0 = 0; o0 < n_owners; o0 += 32) {
         const uint32_t o = o0 + lane;
         if (o >= n_owners) continue;
         const orec_t r = S.orec[o];
         if (or_dead(r) || or_marker(r)) continue;
         uint32_t at = S.opos[o];
-        if (or_line(r) != 1) W.fin[at++] = st_pack(OBM_K_LINE, or_ls(r), or_line(r));
-        W.fin[at] = st_pack(OBM_K_COMMENT, or_first(r), or_slash2(r) ? 2 : 1);
+        if (or_line(r) != 1) fin[at++] = st_pack(OBM_K_LINE, or_ls(r), or_line(r));
+        fin[at] = st_pack(OBM_K_COMMENT, or_first(r), or_slash2(r) ? 2 : 1);
         acc.lexemes++;
     }
     {
@@ -564,12 +573,23 @@ OBMW_DEV bool assemble_fin(WarpSmem &W, UnitSet &S, const UnitRegs &R, WAcc &acc
             const uint32_t ms = S.u.c.mstat[lane]; /* never MS_NONE here: every marker line with tuples is staged */
             if (ms != MS_NONE) { c = ms >> 16; rel = S.opos[S.mlist[lane]]; acc.markers += ms & 0xFFu; acc.lexemes += (ms >> 8) & 0xFFu; }
         }
-        copy_staged(S, ns, c, rel, [&](uint32_t at, uint32_t v) { W.fin[at] = v; });
+        copy_staged(S, ns, c, rel, [&](uint32_t at, uint32_t v) { fin[at] = v; });
     }
-    WSYNC();
+    WSYNC(); /* orders the stores before write_fin's loads by other lanes (shared or global memory alike) */
     return true;
 }
-OBMW_DEV void write_fin(const WarpSmem &W, const WArgs &A, const UnitRegs &R, uint32_t nunits, uint64_t base) {
+/* the words of a deferred unit's fin, lane L holding words k * 32 + L: a whole unit in registers, so that its stores wait for
+ * one round trip to the slot, and the caller issues the loads before chain_resolve so that the two round trips overlap */
+constexpr uint32_t FIN_WORDS = (FIN_CAP + 31) / 32;
+struct FinRegs { uint32_t v[FIN_WORDS]; };
+OBMW_DEV void fin_load(const WarpSmem &W, const WArgs &A, const UnitRegs &R, FinRegs &F) {
+    const uint32_t lane = WLANE();
+    const uint32_t *const fin = W.fin; /* one read of the slot pointer (OBMW_FIN_GLOBAL), not one per load */
+    const bool writing = A.out != nullptr && A.out_cap != 0;
+#pragma unroll
+    for (uint32_t k = 0; k < FIN_WORDS; k++) { const uint32_t f = k * 32 + lane; F.v[k] = writing && f < R.n_small ? fin[f] : 0u; }
+}
+OBMW_DEV void write_fin(const WArgs &A, const UnitRegs &R, uint32_t nunits, uint64_t base, const FinRegs &F) {
     const uint32_t lane = WLANE();
     if (lane == 0) {
         if (R.u == 0) A.tuple_off[0] = 0;
@@ -579,10 +599,18 @@ OBMW_DEV void write_fin(const WarpSmem &W, const WArgs &A, const UnitRegs &R, ui
     if (lane < R.nd) A.tuple_off[R.da + lane + 1] = base + R.dexcl + R.dtot;
     if (A.out != nullptr && A.out_cap != 0) {
         obm_tuple *dst = A.out + base;
-        if (base + R.n_small <= A.out_cap) for (uint32_t f = lane; f < R.n_small; f += 32) dst[f] = st_unpack(W.fin[f]);
-        else for (uint32_t f = lane; f < R.n_small; f += 32) if (base + f < A.out_cap) dst[f] = st_unpack(W.fin[f]);
+        const uint32_t n = R.n_small;
+        const uint64_t room = base < A.out_cap ? A.out_cap - base : 0; /* tuples [0, room) of the unit fit the output */
+#pragma unroll
+        for (uint32_t k = 0; k < FIN_WORDS; k++) { const uint32_t f = k * 32 + lane; if (f < n && f < room) dst[f] = st_unpack(F.v[k]); }
     }
-    WSYNC(); /* fin is free again */
+    WSYNC(); /* fin is free again: the next assemble_fin's stores follow every lane's loads */
+}
+/* both halves at once (the host replay; k_warp_scan puts chain_resolve between them) */
+OBMW_DEV void write_fin(const WarpSmem &W, const WArgs &A, const UnitRegs &R, uint32_t nunits, uint64_t base) {
+    FinRegs F;
+    fin_load(W, A, R, F);
+    write_fin(A, R, nunits, base, F);
 }
 
 /* ---- second half: the unit's tuples at their final positions (base = tuples of all earlier units) ----------
